@@ -29,6 +29,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 PKG = "end-to-end-asr-pytorch_b200"
@@ -47,6 +48,10 @@ def parse_args():
     ap.add_argument("--n-samples", type=int, default=192000)
     ap.add_argument("--cpu-batch", type=int, default=0, help="utterances per CPU-baseline step (0 = auto)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (loss.npy, params.npy) to DIR as float32; the parameters "
+                         "depend on every optimizer step taken before, so two builds compare only with equal arguments "
+                         "and the same cuda_graph outcome")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="time the eager step instead of the CUDA-graph replay")
     ap.add_argument("--no-parity-fp64", action="store_true",
@@ -80,11 +85,11 @@ def peaks():
         with open(path) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -389,7 +394,7 @@ def parity_check(pkg, step_fn, cfg, waves, lens, txt, dev, n_ref=8, fp64=False, 
 
 def micro_bench(pkg, dev, peak):
     """BASELINE.json configs[4]: mel-fbank (+delta+CMVN) and the CTC kernels on 1000 synthetic utterances of 2-30 s
-    (front end: batches of 100; CTC: batches of 250 = 500 lattice warps per launch, enough to occupy the 148 SMs of the
+    (front end: batches of 100; CTC: batches of 250 = 500 lattice warps per launch, enough to occupy the 132 SMs of the
     T'-long latency chain - the train step's batch of 64 is reported by the `kernels` table instead; zero padded to the
     batch maximum), L2 flushed (256 MB write) before every timed launch, CUDA
     events per C-ABI launch.  Algorithmic bytes per SURVEY.md 8(d): fbank 4N + 160m, delta+CMVN 4m(40+120), CTC
@@ -469,6 +474,21 @@ def micro_bench(pkg, dev, peak):
     return out
 
 
+DUMP_MAX_ELEMS = 4 << 20      # 16 MB of float32 per array
+
+
+def dump_outputs(out_dir, loss, params):
+    """What a caller of the timed step holds after its last call: the loss it returned and the parameters it
+    updated in place (a fixed, seeded sample of the flat parameter buffer when that is larger than DUMP_MAX_ELEMS)."""
+    os.makedirs(out_dir, exist_ok=True)
+    flat = params.detach().reshape(-1)
+    if flat.numel() > DUMP_MAX_ELEMS:
+        idx = np.sort(np.random.RandomState(0).choice(flat.numel(), DUMP_MAX_ELEMS, replace=False))
+        flat = flat[torch.from_numpy(idx).to(flat.device)]
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().reshape(1).float().cpu().numpy())
+    np.save(os.path.join(out_dir, "params.npy"), flat.float().cpu().numpy())
+
+
 def main():
     args = parse_args()
     pkg = importlib.import_module(PKG)
@@ -481,11 +501,11 @@ def main():
               "global_batch": per_gpu * world, "per_gpu_batch": per_gpu, "n_samples": args.n_samples,
               "frames": 1 + (args.n_samples - 400) // 160, "vocab": vocab,
               "parallelism": "dp%d (utterance shards; per-layer NCCL grad all-reduce buckets overlapped with backward)" % world,
-              "l2": "inputs+activations per step (>1 GB) exceed the 126 MB L2; no explicit flush",
-              "gemm": "own tcgen05 3xTF32 kernel in three operand forms (x.W^T, dY.W, dY^T.X incl. shifted h_prev reads, split-K, "
-                      "gate permutation in the epilogue), weight residuals (and the wide operand of the weight gradients) pre-split once per step, two-level accumulation (TMEM "
+              "l2": "inputs+activations per step (>1 GB) exceed the 50 MB L2; no explicit flush",
+              "gemm": "own wgmma 3xTF32 kernel in three operand forms (x.W^T, dY.W, dY^T.X incl. shifted h_prev reads, split-K, "
+                      "gate permutation in the epilogue), weight residuals (and the wide operand of the weight gradients) pre-split once per step, two-level accumulation (MMA "
                       "chunks of 128 k summed in fp32 registers); B200ASR_GEMM=tf32x3 selects the cuBLAS 3xTF32 composition; fp32-accurate",
-              "lstm": "tcgen05 fp16 hi/lo 2x2-block split product, forward and backward (H = 256 ... 768; backward exchange: data-is-the-flag polling)"}
+              "lstm": "wgmma fp16 hi/lo 2x2-block split product, forward and backward (H = 256 ... 768; backward exchange: data-is-the-flag polling)"}
 
     # ------------------------------------------------------------------------------- reference (CPU) arm
     if args.impl == "reference":
@@ -505,7 +525,7 @@ def main():
         print(json.dumps(line))
         return 0
 
-    # ------------------------------------------------------------------------------- B200 arm
+    # ------------------------------------------------------------------------------- GPU arm
     assert torch.cuda.is_available(), "bench.py needs a CUDA device (there is no CPU fallback)"
     dp = pkg.dist.DataParallel()
     local = dp.local_rank if dp.enabled else 0
@@ -560,7 +580,7 @@ def main():
         dp.barrier()
         pkg.lib.TIMER.enabled = False
         ms = dp.max_time(a.elapsed_time(b), dev)
-        return ms, float(loss), pkg.lib.launch_count()
+        return ms, loss, pkg.lib.launch_count()
 
     log("warm-up")
     for i in range(max(args.warmup, 3)):
@@ -571,7 +591,7 @@ def main():
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    eager_ms, loss, launches = timed(step_resident, args.steps, profile=True)
+    eager_ms, loss_t, launches = timed(step_resident, args.steps, profile=True)
     summary = pkg.lib.TIMER.summary()
     launches_per_step = launches / args.steps
     log("eager timed region done: %.1f ms/step" % (eager_ms / args.steps))
@@ -592,10 +612,13 @@ def main():
     if use_graph:
         for _ in range(3):
             step_resident()
-        ms, loss, _ = timed(step_resident, args.steps)
+        ms, loss_t, _ = timed(step_resident, args.steps)
     else:
         ms = eager_ms
+    loss = float(loss_t)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss_t, step_fn.optimizer.buf.flat)
     log("timed region done: %.1f ms/step" % (ms / args.steps))
     value = gb * args.steps / (ms / 1000.0)
     e2e = None
@@ -688,23 +711,12 @@ def main():
     if top is not None:
         k = kernels[top]
         d = summary[top]
-        # DRAM traffic per launch = (dram bytes / algorithmic bytes) measured with `ncu --set full` on the SHIPPED kernels
-        # (profiles/r02_ncu_traffic.json, written from this round's captures by tools/ncu_summary.py) x this launch's
-        # algorithmic bytes; null when no capture of that kernel is committed
-        ratios = {}
-        try:
-            with open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")) as f:
-                ratios = json.load(f)
-        except Exception:
-            pass
-        ratio = (ratios.get(top) or {}).get("dram_over_algorithmic")
         alg_per_launch = d["bytes"] / d["launches"]
         roofline = {"kernel": top, "bound": "hbm", "achieved": k["algorithmic_gbs"], "peak": peak, "unit": "GB/s",
-                    "frac": k["frac_hbm"], "traffic": (ratio * alg_per_launch) if ratio else None,
+                    "frac": k["frac_hbm"],
                     "algorithmic_bytes_per_launch": alg_per_launch, "peak_source": peak_src,
-                    "traffic_source": (ratios.get(top) or {}).get("source"),
                     "note": "The LSTM step kernels are bound by the per-step latency chain (gpu-scope fence -> flag -> "
-                            "poll -> bulk copy -> tcgen05 MMAs -> TMEM load -> pointwise), not by HBM (SURVEY.md 7, "
+                            "poll -> bulk copy -> wgmma -> pointwise), not by HBM (SURVEY.md 7, "
                             "AI ~ 170 FLOP/B): see binding_bound"}
         if top.startswith("bilstm"):
             H = cfg["model"]["encoder"]["dim"][0]
@@ -714,19 +726,11 @@ def main():
             tf = flops / (d["ms"] * 1e-3) / 1e12
             us_step = 1e3 * d["ms"] / (steps_dirs / 2.0)
             if lib.b200asr_bilstm_uses_tcgen05(per_gpu, H, 2) == 1:
-                # tensor floor of one step: H/16 MMAs (M 64, N 128) x 64 cycles, measured by tools/micro/umma_probe.cu
-                # (2192 cycles for 32 MMAs incl. completion latency) at the SM clock of this run
-                mhz = (clocks or {}).get("sm_mhz") or 1965.0
-                floor_us = (H / 16.0) * 68.5 / mhz
-                roofline["binding_bound"] = {"bound": "tcgen05 step latency chain", "us_per_recurrent_step": us_step,
-                                             "tensor_floor_us_per_step": floor_us, "frac": floor_us / us_step,
-                                             "achieved": tf, "unit": "TFLOP/s (fp32-equivalent recurrent flops)"}
+                bound = "wgmma step latency chain"
             else:
-                on_tc = lib.b200asr_bilstm_uses_tensor_cores(per_gpu, H, 2) == 1
-                pk = 92.7 if on_tc else 58.0
-                roofline["binding_bound"] = {"bound": "mma_sync_3xtf32" if on_tc else "fp32_fma", "achieved": tf,
-                                             "peak": pk, "unit": "TFLOP/s (fp32-equivalent)", "frac": tf / pk,
-                                             "us_per_recurrent_step": us_step}
+                bound = "mma_sync_3xtf32" if lib.b200asr_bilstm_uses_tensor_cores(per_gpu, H, 2) == 1 else "fp32_fma"
+            roofline["binding_bound"] = {"bound": bound, "us_per_recurrent_step": us_step, "achieved": tf,
+                                         "unit": "TFLOP/s (fp32-equivalent recurrent flops)"}
     line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": config,

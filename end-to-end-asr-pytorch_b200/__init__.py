@@ -1,4 +1,4 @@
-"""b200asr - B200-native (sm_100a) implementation of the End-to-end-ASR-Pytorch train-step hot path.
+"""b200asr - H100-native (sm_90a) implementation of the End-to-end-ASR-Pytorch train-step hot path.
 
 The directory name follows the reference repository; import it with
     importlib.import_module("end-to-end-asr-pytorch_b200")

@@ -1,4 +1,4 @@
-"""Build libb200asr.so in-tree with nvcc for sm_100a (no torch headers, plain C ABI)."""
+"""Build libb200asr.so in-tree with nvcc for sm_90a (no torch headers, plain C ABI)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200asr.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",
 ]
 

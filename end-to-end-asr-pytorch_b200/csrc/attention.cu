@@ -193,8 +193,8 @@ __global__ void __launch_bounds__(1024) locattn_fwd_kernel(AttnParams p) {
 
 // ------------------------------------------------------------------------------------------
 // one thread per attention dim.  MINB = 2 (D <= 384, E / CS <= 512): two CTAs per SM, so that the 256 CTAs of a
-// 64-utterance batch stay ONE wave (measured cfg C: 8.3 vs 10.8 ms per 46 steps); MINB = 1 (D <= 512, E / CS <= 1024):
-// more registers for the value-row prefetch when all CTAs are co-resident anyway (cfg D, 32 utterances: 9.5 vs 11.2 ms).
+// 64-utterance batch stay ONE wave; MINB = 1 (D <= 512, E / CS <= 1024):
+// more registers for the value-row prefetch when all CTAs are co-resident anyway (cfg D, 32 utterances).
 template <int MINB>
 __global__ void __launch_bounds__(MINB == 2 ? 384 : 512, MINB) locattn_bwd_kernel(AttnParams p) {
     extern __shared__ __align__(16) float sm[];

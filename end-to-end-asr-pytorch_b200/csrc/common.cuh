@@ -1,4 +1,4 @@
-// Shared helpers for the b200asr sm_100a kernels (error plumbing, launch accounting, warp/block
+// Shared helpers for the b200asr sm_90a kernels (error plumbing, launch accounting, warp/block
 // reductions, mbarrier + bulk-copy wrappers).  Everything in csrc/ is compiled into ONE shared
 // library (libb200asr.so) whose only exported symbols are the extern "C" entry points declared in
 // include/b200asr.h.

@@ -23,8 +23,8 @@ static int query_attr(cudaDeviceAttr attr, int fallback) {
     if (cudaDeviceGetAttribute(&v, attr, dev) != cudaSuccess) { cudaGetLastError(); return fallback; }
     return v > 0 ? v : fallback;
 }
-// B200 defaults when no device is visible (host-only planning / symbol tests)
-int sm_count() { return query_attr(cudaDevAttrMultiProcessorCount, 148); }
+// H100 (SXM) defaults when no device is visible (host-only planning / symbol tests)
+int sm_count() { return query_attr(cudaDevAttrMultiProcessorCount, 132); }
 int max_optin_smem() { return query_attr(cudaDevAttrMaxSharedMemoryPerBlockOptin, 232448); }
 
 }  // namespace b200asr

@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(1024) ctc_alpha_beta_kernel(CtcParams p) {
         // one lattice position per thread (every target shorter than 512 labels): the emission gathers run PD frames
         // ahead in a register ring, off the T-long dependency chain.  The ring holds the RAW loads (logit and row lse);
         // the subtraction happens at the consumer - an FADD next to the load makes the warp wait for the gather right
-        // there.  (The cp.async ring of the warp kernel was measured here too: 25 % slower with a barrier per frame.)
+        // there.  (The cp.async ring of the warp kernel would need a block barrier per frame here.)
         constexpr int PD = 4;
         const int s = threadIdx.x;
         const bool act = s < Sb;
@@ -408,10 +408,8 @@ __global__ void __launch_bounds__(CTC_WARPS * 32) ctc_alpha_beta_warp_kernel(Ctc
     const int dt = is_beta ? -1 : 1;
     // The emission gathers x[t, label] are independent of the recursion: they run CTC_PD frames ahead as cp.async copies
     // into a per-warp shared-memory ring, one commit group per frame; every lane reads back only what it copied itself.
-    // Measured at V = 5000 (1000 utterances, L2 flushed): register ring with the "- lse" next to the load 2.31 ms (the
-    // FADD stalls on the load it follows), register ring of raw loads 1.49 ms, this ring 1.30 ms.  What is left is the
-    // recursion itself: ~300 dependent instructions per frame in a single warp (ncu: top stall `wait`, long_scoreboard
-    // 0.09 warps per issue - profiles/r02_ncu_misc.txt).
+    // (A register ring with the "- lse" next to the load stalls the FADD on the load it follows.)  What is left is the
+    // recursion itself: ~300 dependent instructions per frame in a single warp.
     float a[R];
     const float* lseb = p.lse ? p.lse + (long long)b * p.T : nullptr;
     auto prefetch = [&](int st) {                        // frame t0 + dt * st -> ring slot st % CTC_PD
@@ -710,8 +708,8 @@ static int ctc_fwd_bwd_impl(const float* log_probs, const float* row_lse, long l
     if (rc != B200_OK) return rc;
     const int need = (p.S_max + 31) / 32;      // extended-label positions per lane
     // The warp-synchronous kernel wins while a lane holds few positions (subword targets: S <= 128); for long
-    // character targets one position per thread + a block barrier is faster (measured: V=31, L~130: 3.7 vs 9.1 ms
-    // per 1000 utterances), so those take the block kernel.
+    // character targets one position per thread + a block barrier is faster (V = 31, L ~ 130), so those
+    // take the block kernel.
     if (need <= 4 && (size_t)CTC_WARPS * 2 * p.S_max * sizeof(float) <= 48 * 1024) {
         if (need <= 1) launch_ctc_warp<1>(p, (cudaStream_t)stream);
         else if (need <= 2) launch_ctc_warp<2>(p, (cudaStream_t)stream);

@@ -228,8 +228,7 @@ __device__ __forceinline__ float delta_value(const DeltaParams& p, const float* 
 // The chunk's fbank rows [t0 - pad, t0 + DC_TCHUNK + pad) are staged ONCE in shared memory (zeros outside [0, m): the
 // zero padding of src/audio.py:57-77) together with the tap weights; the taps then read shared memory.  Same tap order
 // and the same fmaf chain as delta_value() above (a zero tap or a zero-padded row adds exactly 0), so the values are
-// bit-identical to the round-1 kernels that re-read global memory per tap (measured 0.05 of HBM: ~25 instructions per
-// tap, branchy).
+// bit-identical to a kernel that re-reads global memory per tap (~25 instructions per tap, branchy).
 __device__ __forceinline__ void delta_stage(const DeltaParams& p, const float* fb, int m, int t0, float* s_fb,
                                             float* s_filt) {
     const int rows = DC_TCHUNK + p.taps - 1;

@@ -1,4 +1,4 @@
-// K6 / K9 / K11: the dense contractions of the step on the 5th-generation tensor cores, fp32 in and out, fp32-class
+// K6 / K9 / K11: the dense contractions of the step on the Hopper tensor cores (wgmma), fp32 in and out, fp32-class
 // accuracy ("3xTF32").  ONE kernel template serves the three operand arrangements of a layer y = x . W^T + b:
 //   tn :  C[M,N] (+)= A[M,K] . B[N,K]^T + bias      forward  (x . W^T): both operands K-major (K contiguous)
 //   nn :  C[M,N] (+)= A[M,K] . B[K,N]               input gradient (dY . W): B is MN-major (N contiguous)
@@ -10,55 +10,48 @@
 //   reference call sites: the input projection inside nn.LSTM (src/module.py:112-113,131), the CTC head (src/asr.py:29,
 //   96), proj_k / char_trans / pj (src/asr.py:242-243,177,220; src/module.py:123,155) and their autograd backward.
 //
-// tcgen05.mma kind::tf32 reads fp32 bit patterns from shared memory and IGNORES the low 13 mantissa bits (truncation,
-// verified on hardware by tools/micro/umma_probe.cu), so the raw fp32 tile IS the TF32 "hi" operand - no split pass,
-// no second copy in HBM.  Only the residual  lo = x - trunc(x)  has to exist as its own tile, and it has the same
-// shared-memory layout as the raw tile, so making it is a purely elementwise pass by 8 "splitter" warps.  Per 32-wide
-// K block the single-thread issuer then accumulates   A.B + A_lo.B + A.B_lo   in one TMEM accumulator (fp32).
+// wgmma .tf32 reads fp32 bit patterns from shared memory and ignores the low 13 mantissa bits (inferred from the fp32-
+// class parity tests of the tn form, which only hold if the hardware truncates; not probed in isolation), so a raw
+// K-major fp32 tile IS the TF32 "hi" operand; the residual  lo = x - trunc(x)  is a second tile of the same layout.  Per 32-wide K
+// block the two consumer warpgroups accumulate  A.B + A_lo.B + A.B_lo  in one fp32 register accumulator.
+// wgmma has no MN-major form for 32-bit types: an MN-major operand is loaded as plain [32 k][32 column] boxes and
+// transposed into the K-major swizzled image (hi and lo at once) by the same pass that makes the residuals.
 //
-// One 128 x 256 tile per CTA (x split-K slices when the tile grid alone cannot fill the SMs: partial tiles go to a
+// One 128 x 128 tile per CTA (x split-K slices when the tile grid alone cannot fill the SMs: partial tiles go to a
 // workspace and a second small kernel sums them in a fixed order - deterministic).  Warp roles: 0 = TMA producer
-// (cp.async.bulk.tensor, 128-byte swizzle, out-of-bounds rows / K tail zero-filled by the hardware), 1 = MMA issue +
-// TMEM allocation, 2..9 = splitters, which also own the second accumulation level: the TMEM chain is cut every 4 K
-// blocks, the partial tile is drained (tcgen05.ld 32x32b) into 128 fp32 registers per thread and summed there, while
-// the tensor core fills the other of two TMEM buffers; the epilogue (+ bias [+ C], 128-bit stores) runs from those
-// registers.  Two shared-memory stages of 96 KB (A 16 + B 32 raw, the same again for the residuals).
-//
-// What bounds it (measured, profiles/r02_ncu_lstm_gemm.txt + tools/time_gemm.py): shared-memory bandwidth.  Per 32-wide
-// K block the tensor core reads 12 x (4 + 8) KB of operands, TMA writes 48 KB and the splitters read and write 48 KB
-// each = 288 KB ~ 2250 cycles at 128 B/clk against 1536 cycles of MMA time: 225 TFLOP/s fp32-equivalent (675 TF/s of
-// TF32 issue, ~60 % of the pipe; ncu: tensor pipe 45-50 % active at M = 8192) - on par with the three cuBLAS TF32 GEMMs
-// + split passes it replaces (tools/time_gemm.py).  Tried and rejected: three raw stages with a single residual
-// buffer (the splitter pass, ~1300 cycles, then serialises with the cross products: 187 TFLOP/s).
+// (cp.async.bulk.tensor, out-of-bounds rows / K tail zero-filled by the hardware), 4..11 = two consumer warpgroups
+// (64 rows each): they split K block i+1 while their asynchronous MMAs of K block i run.  The accumulation chain is cut
+// every G_CH K blocks and summed with IEEE fp32 adds in a second register tile (the tensor core's fp32 accumulate
+// is not IEEE-rounded); the epilogue (+ bias [+ C]) runs from those registers.
 //
 // Shared-memory images.  K-major operand, R rows: R consecutive 128-byte rows (32 k each), 128-byte swizzle; one MMA
-// (8 k) advances the descriptor start by 32 bytes.  MN-major operand, R columns: R/32 boxes of [32 k][32 columns] =
-// 4096 bytes each (a TMA box {32 columns, 32 rows}); for 32-bit types the tensor core wants the 128-byte swizzle with
-// a 32-byte base (TMA SWIZZLE_128B_ATOM_32B <-> descriptor layout SWIZZLE_128B_BASE32B), LBO = 4096 B (next 32
-// columns), SBO = 512 B (next 4 k); one MMA (8 k) advances the start by 1024 bytes.
+// (8 k) advances the descriptor start by 32 bytes.  MN-major operand as loaded: R/32 boxes of [32 k][32 columns] =
+// 4096 bytes each (a TMA box {32 columns, 32 rows}, no swizzle).
 #include <cuda.h>
 #include <stdlib.h>
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 #include "../../include/b200asr.h"
 
 namespace b200asr {
 namespace {
 
-constexpr int G_BM = 128, G_BN = 256, G_BK = 32;
-constexpr int G_STAGES = 2;
-constexpr int G_A_BYTES = G_BM * G_BK * 4;      // 16 KB
-constexpr int G_B_BYTES = G_BN * G_BK * 4;      // 32 KB
-constexpr int G_STAGE_BYTES = 2 * (G_A_BYTES + G_B_BYTES);
-constexpr int G_SPLIT_WARPS = 8;
-constexpr int G_THREADS = 32 * (2 + G_SPLIT_WARPS);
+constexpr int G_BM = 128, G_BN = 128, G_BK = 32;
+constexpr int G_TILE = G_BM * G_BK * 4;         // 16 KB: one operand tile (G_BM == G_BN)
+constexpr int G_CONSUMERS = 256;                // two warpgroups
+constexpr int G_THREADS = 128 + G_CONSUMERS;    // warpgroup 0: TMA producer (one lane)
 constexpr int G_BOX = 32 * G_BK * 4;            // one MN-major box: 32 columns x 32 k
 constexpr int G_MAX_SPLIT = 32;
-#ifndef B200ASR_GEMM_HH_FIRST
-#define B200ASR_GEMM_HH_FIRST 1     // measured +1.7 % (228 vs 224.5 TFLOP/s at M = 38k, N = K = 2048)
-#endif
-constexpr bool HH_FIRST = B200ASR_GEMM_HH_FIRST != 0;   // issue the hi.hi products before the residual tiles are ready
-constexpr int G_CH_DEFAULT = 4;              // K blocks per TMEM accumulation chunk (see the drain warps); 1, 2 or 4
+constexpr int G_CH_DEFAULT = 4;                 // K blocks per accumulation chunk; 1, 2 or 4
+
+// stage: [A as loaded | B as loaded | A lo | B lo | A hi (K-major image, MN-major A only) | B hi (same for B)]
+template <bool A_MN, bool B_MN>
+struct GemmSmem {
+    static constexpr int STAGE = (4 + (A_MN ? 1 : 0) + (B_MN ? 1 : 0)) * G_TILE;
+    static constexpr int STAGES = (A_MN || B_MN) ? 2 : 3;
+    static constexpr int A_HI = A_MN ? 4 * G_TILE : 0;
+    static constexpr int B_HI = B_MN ? (A_MN ? 5 : 4) * G_TILE : G_TILE;
+};
 
 struct GemmArgs {
     const float* bias;
@@ -69,7 +62,7 @@ struct GemmArgs {
     int kb_per_split;
     int kbt;               // K blocks per batch entry (MN-major operands walk (batch, time)); KB = batches * kbt
     int a_shift, b_shift;  // time shift of the rows read from A / B (nt form)
-    int ch;                // K blocks per TMEM accumulation chunk
+    int ch;                // K blocks per accumulation chunk
 };
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
@@ -90,44 +83,46 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 __device__ __forceinline__ void g_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ float tf32_residual(float x) {
-    return x - __uint_as_float(__float_as_uint(x) & 0xffffe000u);
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(G_CONSUMERS) : "memory"); }
+__device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
+__device__ __forceinline__ float tf32_residual(float x) { return x - tf32_trunc(x); }
+
+// Residual of a K-major tile (elementwise: the image keeps its layout).
+__device__ __forceinline__ void split_k_tile(const uint8_t* raw, uint8_t* lo, int ct) {
+    const float4* src = reinterpret_cast<const float4*>(raw);
+    float4* dst = reinterpret_cast<float4*>(lo);
+#pragma unroll 4
+    for (int j = ct; j < G_TILE / 16; j += G_CONSUMERS) {
+        const float4 v = src[j];
+        dst[j] = make_float4(tf32_residual(v.x), tf32_residual(v.y), tf32_residual(v.z), tf32_residual(v.w));
+    }
 }
-// MN-major matrix descriptor for a 32-bit type: the tensor core transposes 32-bit MN-major operands at 32-byte
-// granularity, so the layout type is SWIZZLE_128B_BASE32B (= 1: 32-byte chunks swizzled within the 128-byte row, pattern
-// period 4 rows - what a TMA load with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B produces).  Leading byte offset = distance
-// between 32-column boxes, stride byte offset = distance between groups of 4 k (512 bytes).
-__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t smem_addr) {
-    uint64_t d = static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-    d |= static_cast<uint64_t>(G_BOX >> 4) << 16;
-    d |= static_cast<uint64_t>(512 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(1) << 61;
-    return d;
+// [32 k][32 column] boxes -> K-major swizzled hi and lo images: warp w moves k = 4w .. 4w+3 of column `lane`.
+__device__ __forceinline__ void split_mn_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int boxes, int ct) {
+    const int c = ct & 31, k0 = (ct >> 5) * 4;
+    for (int j = 0; j < boxes; ++j) {
+        const float* b = reinterpret_cast<const float*>(raw + j * G_BOX) + k0 * 32 + c;
+        const float x0 = b[0], x1 = b[32], x2 = b[64], x3 = b[96];
+        const uint32_t off = wgmma::sw128_offset(32 * j + c, k0 * 4);
+        *reinterpret_cast<float4*>(hi + off) = make_float4(tf32_trunc(x0), tf32_trunc(x1), tf32_trunc(x2), tf32_trunc(x3));
+        *reinterpret_cast<float4*>(lo + off) =
+            make_float4(tf32_residual(x0), tf32_residual(x1), tf32_residual(x2), tf32_residual(x3));
+    }
 }
 
-// B_PRE: the residual tile of B comes from a pre-computed residual matrix (same shape / layout as B: the weights, split
-// once per step by b200asr_tf32_residual) through its own tensor map, so the splitters only pass over the A tile and the
-// issuer can run  A.B  and  A.B_lo  (8 of the 12 MMAs of a K block) as soon as the TMA has landed.
-// A_PRE: the same for A (an activation / gradient matrix whose residual the caller made once and uses in several
-// products).  With both, the splitters have nothing to split: all 12 MMAs of a K block are issued when the TMA has
-// landed and shared memory sees 240 KB of traffic per K block instead of 288.  Measured SLOWER than B_PRE alone
-// (tn 248 -> 232, nn 233 -> 208 TFLOP/s, nt unchanged at 180): per K block the SM then takes in 96 KB through TMA
-// instead of 80 (64 without any pre-split), and the L2 -> SM path (measured ceiling ~45-50 B/clk/SM,
-// tools/micro/xfer_probe.cu; 33 B/clk/SM at 248 TFLOP/s) is the tighter resource.  Kept as a tested option; the step
-// uses B_PRE (weights) only.  What would lift this bound is a CTA pair sharing the B tile (cta_group::2).
+// B_PRE / A_PRE: the residual of a K-major operand comes from a pre-computed residual matrix (same shape / layout: the
+// weights, split once per step by b200asr_tf32_residual) through its own tensor map, so the consumers do not pass
+// over that tile.  K-major operands only: an MN-major operand goes through the transposing pass, which makes its
+// residual in the same sweep.
 template <bool A_MN, bool B_MN, bool B_PRE, bool A_PRE>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
               const __grid_constant__ CUtensorMap map_blo, const __grid_constant__ CUtensorMap map_alo, const GemmArgs g) {
+    using L = GemmSmem<A_MN, B_MN>;
+    static_assert(!(A_PRE && A_MN) && !(B_PRE && B_MN), "only K-major operands bring a pre-computed residual");
     extern __shared__ __align__(1024) uint8_t smem[];
-    // stage s: [A raw | B raw | A lo | B lo]
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + G_STAGES * G_STAGE_BYTES);   // TMA landed
-    uint64_t* split = full + G_STAGES;                                               // residual tiles written
-    uint64_t* empty = split + G_STAGES;                                              // MMAs of the stage retired
-    uint64_t* acc_full = empty + G_STAGES;                                           // [2] a chunk's MMAs retired
-    uint64_t* acc_free = acc_full + 2;                                               // [2] the chunk has been drained
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_free + 2);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + L::STAGES * L::STAGE);      // TMA landed
+    uint64_t* empty = full + L::STAGES;                                              // MMAs of the stage retired
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m0 = blockIdx.y * G_BM, n0 = blockIdx.x * G_BN;
@@ -135,40 +130,27 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
     const int kb0 = blockIdx.z * g.kb_per_split;
     const int kb1 = min(g.KB, kb0 + g.kb_per_split);
     const int nkb = kb1 - kb0;                                   // >= 1 by construction of the grid
-    const int G_CH = g.ch;
-    const int nchunks = (nkb + G_CH - 1) / G_CH;
-    const int nvalid = min(G_BN, N - n0);
-    const int n_instr = (nvalid + 15) & ~15;                     // MMA N (multiple of 16, <= 256)
     const int a_boxes = min(G_BM / 32, (M - m0 + 31) / 32);      // MN-major: 32-column boxes that hold real data
-    const int b_boxes = (nvalid + 31) / 32;
-    const uint32_t a_bytes = A_MN ? (uint32_t)a_boxes * G_BOX : (uint32_t)G_A_BYTES;
-    const uint32_t b_bytes = B_MN ? (uint32_t)b_boxes * G_BOX : (uint32_t)G_B_BYTES;
+    const int b_boxes = min(G_BN / 32, (N - n0 + 31) / 32);
+    const uint32_t a_bytes = A_MN ? (uint32_t)a_boxes * G_BOX : (uint32_t)G_TILE;
+    const uint32_t b_bytes = B_MN ? (uint32_t)b_boxes * G_BOX : (uint32_t)G_TILE;
 
     if (tid == 0) {
-        for (int s = 0; s < G_STAGES; ++s) {
+        for (int s = 0; s < L::STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&split[s], G_SPLIT_WARPS);
-            mbar_init(&empty[s], 1);
-        }
-        for (int j = 0; j < 2; ++j) {
-            mbar_init(&acc_full[j], 1);
-            mbar_init(&acc_free[j], G_SPLIT_WARPS);
+            mbar_init(&empty[s], G_CONSUMERS / 32);
         }
         mbar_fence_init();
     }
-    if (warp == 1) umma::tmem_alloc(tmem_slot, 512);
-    umma::fence_before_sync();
     __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem = *tmem_slot;
 
     if (warp == 0) {
         if (lane == 0) {
             for (int i = 0; i < nkb; ++i) {
                 const int kb = kb0 + i;
-                const int s = i % G_STAGES;
-                if (i >= G_STAGES) mbar_wait(&empty[s], (uint32_t)(((i / G_STAGES) - 1) & 1));
-                uint8_t* st = smem + s * G_STAGE_BYTES;
+                const int s = i % L::STAGES;
+                if (i >= L::STAGES) mbar_wait(&empty[s], (uint32_t)(((i / L::STAGES) - 1) & 1));
+                uint8_t* st = smem + s * L::STAGE;
                 mbar_expect_tx(&full[s], (A_PRE ? 2 * a_bytes : a_bytes) + (B_PRE ? 2 * b_bytes : b_bytes));
                 const int bt = kb / g.kbt, t0 = (kb - bt * g.kbt) * G_BK;
                 if (A_MN) {
@@ -176,182 +158,89 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
                         tma_load_3d(st + j * G_BOX, &map_a, m0 + 32 * j, t0 + g.a_shift, bt, &full[s]);
                 } else {
                     tma_load_2d(st, &map_a, kb * G_BK, m0, &full[s]);
+                    if (A_PRE) tma_load_2d(st + 2 * G_TILE, &map_alo, kb * G_BK, m0, &full[s]);
                 }
                 if (B_MN) {
                     for (int j = 0; j < b_boxes; ++j)
-                        tma_load_3d(st + G_A_BYTES + j * G_BOX, &map_b, n0 + 32 * j, t0 + g.b_shift, bt, &full[s]);
+                        tma_load_3d(st + G_TILE + j * G_BOX, &map_b, n0 + 32 * j, t0 + g.b_shift, bt, &full[s]);
                 } else {
-                    tma_load_2d(st + G_A_BYTES, &map_b, kb * G_BK, n0, &full[s]);
-                }
-                if (A_PRE) {                                   // residual of A -> the "A lo" slot of the stage
-                    uint8_t* lo = st + G_A_BYTES + G_B_BYTES;
-                    if (A_MN) {
-                        for (int j = 0; j < a_boxes; ++j)
-                            tma_load_3d(lo + j * G_BOX, &map_alo, m0 + 32 * j, t0 + g.a_shift, bt, &full[s]);
-                    } else {
-                        tma_load_2d(lo, &map_alo, kb * G_BK, m0, &full[s]);
-                    }
-                }
-                if (B_PRE) {                                   // residual of B -> the "B lo" slot of the stage
-                    uint8_t* lo = st + G_A_BYTES + G_B_BYTES + G_A_BYTES;
-                    if (B_MN) {
-                        for (int j = 0; j < b_boxes; ++j)
-                            tma_load_3d(lo + j * G_BOX, &map_blo, n0 + 32 * j, t0 + g.b_shift, bt, &full[s]);
-                    } else {
-                        tma_load_2d(lo, &map_blo, kb * G_BK, n0, &full[s]);
-                    }
+                    tma_load_2d(st + G_TILE, &map_b, kb * G_BK, n0, &full[s]);
+                    if (B_PRE) tma_load_2d(st + 3 * G_TILE, &map_blo, kb * G_BK, n0, &full[s]);
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = umma::instr_desc(umma::FMT_TF32, G_BM, n_instr) | (A_MN ? (1u << 15) : 0u) |
-                                   (B_MN ? (1u << 16) : 0u);
-            for (int i = 0; i < nkb; ++i) {
-                const int s = i % G_STAGES;
-                const int c = i / G_CH, j = i - c * G_CH, buf = c & 1;
-                if (j == 0 && c >= 2) {                       // the drain warps have read chunk c-2 out of this buffer
-                    mbar_wait(&acc_free[buf], (uint32_t)(((c >> 1) - 1) & 1));
-                    umma::fence_after_sync();
-                }
-                const uint32_t d = tmem + 256u * buf;
-                const uint32_t a = smem_u32(smem + s * G_STAGE_BYTES), b = a + G_A_BYTES;
-                const uint32_t alo = b + G_B_BYTES, blo = alo + G_A_BYTES;
-                if (HH_FIRST || B_PRE || A_PRE) {
-                    // the hi.hi products need the raw tiles only (and A.B_lo too when B's residual came by TMA): issue
-                    // them when the TMA has landed, so that the splitters' pass overlaps tensor-core work
-                    mbar_wait(&full[s], (uint32_t)((i / G_STAGES) & 1));
-                    umma::fence_after_sync();
-#pragma unroll
-                    for (int k4 = 0; k4 < G_BK / 8; ++k4) {
-                        const uint64_t da = A_MN ? desc_mn_sw128(a + k4 * 1024) : umma::desc_k_sw128(a + k4 * 32);
-                        const uint64_t db = B_MN ? desc_mn_sw128(b + k4 * 1024) : umma::desc_k_sw128(b + k4 * 32);
-                        umma::mma_ss<umma::FMT_TF32>(d, da, db, idesc, (j | k4) != 0);
-                        if (B_PRE) {
-                            const uint64_t dbl = B_MN ? desc_mn_sw128(blo + k4 * 1024) : umma::desc_k_sw128(blo + k4 * 32);
-                            umma::mma_ss<umma::FMT_TF32>(d, da, dbl, idesc, 1);
-                        }
-                        if (A_PRE) {
-                            const uint64_t dal = A_MN ? desc_mn_sw128(alo + k4 * 1024) : umma::desc_k_sw128(alo + k4 * 32);
-                            umma::mma_ss<umma::FMT_TF32>(d, dal, db, idesc, 1);
-                        }
-                    }
-                }
-                if (!(A_PRE && B_PRE)) {
-                    mbar_wait(&split[s], (uint32_t)((i / G_STAGES) & 1));
-                    umma::fence_after_sync();
-#pragma unroll
-                    for (int k4 = 0; k4 < G_BK / 8; ++k4) {
-                        const uint64_t da = A_MN ? desc_mn_sw128(a + k4 * 1024) : umma::desc_k_sw128(a + k4 * 32);
-                        const uint64_t db = B_MN ? desc_mn_sw128(b + k4 * 1024) : umma::desc_k_sw128(b + k4 * 32);
-                        const uint64_t dal = A_MN ? desc_mn_sw128(alo + k4 * 1024) : umma::desc_k_sw128(alo + k4 * 32);
-                        const uint64_t dbl = B_MN ? desc_mn_sw128(blo + k4 * 1024) : umma::desc_k_sw128(blo + k4 * 32);
-                        if (!HH_FIRST && !B_PRE && !A_PRE) umma::mma_ss<umma::FMT_TF32>(d, da, db, idesc, (j | k4) != 0);
-                        if (!A_PRE) umma::mma_ss<umma::FMT_TF32>(d, dal, db, idesc, 1);
-                        if (!B_PRE) umma::mma_ss<umma::FMT_TF32>(d, da, dbl, idesc, 1);
-                    }
-                }
-                umma::commit(&empty[s]);
-                if (j == G_CH - 1 || i == nkb - 1) umma::commit(&acc_full[buf]);
-            }
-        }
-    } else {
-        // ------------------------------------------- splitters (lo = x - trunc_tf32(x)) + second-level accumulation
-        // The tensor core ADDS into its fp32 accumulator with truncation (measured: a bias of ~2^-25.5 of the running
-        // sum per MMA, always towards zero, i.e. linear in K).  The TMEM chain is therefore cut into chunks of G_CH
-        // K blocks (48 MMAs); each chunk's partial tile is drained into registers and summed there with IEEE fp32
-        // adds, while the tensor core already fills the other TMEM buffer.
-        const int st_tid = tid - 64;                                  // 0..255
-        const int q = warp & 3, half = (warp - 2) >> 2;               // TMEM lane quadrant, column half of the tile
-        const uint32_t t_base = tmem + ((uint32_t)(32 * q) << 16) + 128u * half;
-        float acc[128];
-#pragma unroll
-        for (int e = 0; e < 128; ++e) acc[e] = 0.f;
-        int next_drain = 0;
-        auto drain = [&](int c) {
-            const int buf = c & 1;
-            mbar_wait(&acc_full[buf], (uint32_t)((c >> 1) & 1));
-            umma::fence_after_sync();
-#pragma unroll
-            for (int gq = 0; gq < 4; ++gq) {
-                uint32_t v[32];
-                umma::ld_32x32b_x32(t_base + 256u * buf + 32u * gq, v);
-                umma::wait_ld();
-#pragma unroll
-                for (int e = 0; e < 32; ++e) acc[32 * gq + e] += __uint_as_float(v[e]);
-            }
-            umma::fence_before_sync();
-            __syncwarp();
-            if (lane == 0) g_arrive(&acc_free[buf]);
+    } else if (warp >= 4) {
+        const int ct = tid - 128, wg = ct >> 7;
+        auto split = [&](int i) {
+            const int s = i % L::STAGES;
+            mbar_wait(&full[s], (uint32_t)((i / L::STAGES) & 1));
+            uint8_t* st = smem + s * L::STAGE;
+            if (A_MN) split_mn_tile(st, st + L::A_HI, st + 2 * G_TILE, a_boxes, ct);
+            else if (!A_PRE) split_k_tile(st, st + 2 * G_TILE, ct);
+            if (B_MN) split_mn_tile(st + G_TILE, st + L::B_HI, st + 3 * G_TILE, b_boxes, ct);
+            else if (!B_PRE) split_k_tile(st + G_TILE, st + 3 * G_TILE, ct);
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> the tensor core
         };
-        // only the bytes that were loaded: A tile (or its valid boxes) and B tile (or its valid boxes)
-        const int a_vec = A_PRE ? 0 : (int)(a_bytes / 16), b_vec = B_PRE ? 0 : (int)(b_bytes / 16);
+        float acc[64], d[64];
+#pragma unroll
+        for (int e = 0; e < 64; ++e) acc[e] = 0.f;
+        split(0);
+        consumer_sync();
         for (int i = 0; i < nkb; ++i) {
-            const int s = i % G_STAGES;
-            mbar_wait(&full[s], (uint32_t)((i / G_STAGES) & 1));
-            const float4* src = reinterpret_cast<const float4*>(smem + s * G_STAGE_BYTES);
-            float4* dst = reinterpret_cast<float4*>(smem + s * G_STAGE_BYTES + G_A_BYTES + G_B_BYTES);
-#pragma unroll 4
-            for (int j = st_tid; j < a_vec; j += 32 * G_SPLIT_WARPS) {
-                const float4 v = src[j];
-                dst[j] = make_float4(tf32_residual(v.x), tf32_residual(v.y), tf32_residual(v.z), tf32_residual(v.w));
+            const int s = i % L::STAGES, j = i % g.ch;
+            const uint32_t st = smem_u32(smem + s * L::STAGE);
+            const uint32_t a = st + L::A_HI + wg * (64 * 128), alo = st + 2 * G_TILE + wg * (64 * 128);
+            const uint32_t b = st + L::B_HI, blo = st + 3 * G_TILE;
+            wgmma::fence_operand(d);
+            wgmma::fence();
+#pragma unroll
+            for (int k4 = 0; k4 < G_BK / 8; ++k4) {
+                const uint64_t da = wgmma::desc_k_sw128(a + k4 * 32), db = wgmma::desc_k_sw128(b + k4 * 32);
+                wgmma::mma_tf32_n128(d, da, db, (j | k4) != 0);
+                wgmma::mma_tf32_n128(d, wgmma::desc_k_sw128(alo + k4 * 32), db, 1);
+                wgmma::mma_tf32_n128(d, da, wgmma::desc_k_sw128(blo + k4 * 32), 1);
             }
-#pragma unroll 4
-            for (int j = G_A_BYTES / 16 + st_tid; j < G_A_BYTES / 16 + b_vec; j += 32 * G_SPLIT_WARPS) {
-                const float4 v = src[j];
-                dst[j] = make_float4(tf32_residual(v.x), tf32_residual(v.y), tf32_residual(v.z), tf32_residual(v.w));
+            wgmma::commit_group();
+            if (i + 1 < nkb) split(i + 1);                 // overlaps the MMAs of K block i
+            wgmma::wait_all();
+            wgmma::fence_operand(d);
+            if (lane == 0) g_arrive(&empty[s]);
+            if (j == g.ch - 1 || i == nkb - 1) {
+#pragma unroll
+                for (int e = 0; e < 64; ++e) acc[e] += d[e];
             }
-            if (!(A_PRE && B_PRE)) {                      // (nothing was written and nobody waits otherwise)
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) g_arrive(&split[s]);
-            }
-            // chunk i/G_CH - 1 retired at the latest when K block i-2 left the 2-stage ring: drain it now
-            if (i > G_CH && ((i - 1) % G_CH) == 0) drain(next_drain++);
+            consumer_sync();                               // every thread's split of K block i+1 is in place
         }
-        while (next_drain < nchunks) drain(next_drain++);
         // ---------------------------------------------------------------- epilogue: registers -> C
-        {
-            const int row = m0 + 32 * q + lane;
-            const bool to_partial = gridDim.z > 1;
-            float* Cb = to_partial ? g.partial + (size_t)blockIdx.z * M * N : g.C;
-            const int ldc = to_partial ? N : g.ldc;
+        const bool to_partial = gridDim.z > 1;
+        float* Cb = to_partial ? g.partial + (size_t)blockIdx.z * M * N : g.C;
+        const int ldc = to_partial ? N : g.ldc;
+        const float* bias = to_partial ? nullptr : g.bias;
+        const int accumulate = to_partial ? 0 : g.accumulate;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = m0 + 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+            if (row >= M) continue;
             const int orow = (!to_partial && g.perm) ? (row & 3) * (M >> 2) + (row >> 2) : row;
-            const float* bias = to_partial ? nullptr : g.bias;
-            const int accumulate = to_partial ? 0 : g.accumulate;
-            const bool vec = ((ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(Cb) & 15) == 0);
-            if (row < M) {
-                float* crow = Cb + (size_t)orow * ldc + n0 + 128 * half;
+            float* crow = Cb + (size_t)orow * ldc;
+            const bool vec = ((ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(Cb) & 7) == 0);
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int n = n0 + 128 * half + 4 * j;
-                    if (n < N) {
-                        float o[4];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            o[e] = acc[4 * j + e];
-                            if (bias && n + e < N) o[e] += bias[n + e];
-                        }
-                        if (vec && n + 3 < N) {
-                            float4* p4 = reinterpret_cast<float4*>(crow + 4 * j);
-                            if (accumulate) {
-                                const float4 old = *p4;
-                                o[0] += old.x; o[1] += old.y; o[2] += old.z; o[3] += old.w;
-                            }
-                            *p4 = make_float4(o[0], o[1], o[2], o[3]);
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 4; ++e)
-                                if (n + e < N) crow[4 * j + e] = accumulate ? crow[4 * j + e] + o[e] : o[e];
-                        }
-                    }
+            for (int gq = 0; gq < 16; ++gq) {
+                const int n = n0 + 8 * gq + 2 * (lane & 3);
+                float o0 = acc[4 * gq + 2 * h], o1 = acc[4 * gq + 2 * h + 1];
+                if (bias && n < N) o0 += bias[n];
+                if (bias && n + 1 < N) o1 += bias[n + 1];
+                if (vec && n + 1 < N) {
+                    float2* p2 = reinterpret_cast<float2*>(crow + n);
+                    if (accumulate) { const float2 old = *p2; o0 += old.x; o1 += old.y; }
+                    *p2 = make_float2(o0, o1);
+                } else {
+                    if (n < N) crow[n] = accumulate ? crow[n] + o0 : o0;
+                    if (n + 1 < N) crow[n + 1] = accumulate ? crow[n + 1] + o1 : o1;
                 }
             }
         }
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 1) umma::tmem_dealloc(tmem, 512);
 }
 
 // C[perm(m)][n] (+)= bias[n] + sum_s partial[s][m][n]   (fixed summation order)
@@ -421,16 +310,16 @@ int make_map_k(CUtensorMap* map, const float* ptr, int rows, int K, int ld, int 
 }
 
 // MN-major operand: element (batch b, time t, column c) at ptr[b * bstride + t * ld + c] -> 3-D tensor map (c, t, b)
-// with boxes of 32 columns x 32 rows x 1, 128-byte swizzle; reads outside [0,cols) x [0,T) are zero-filled
+// with boxes of 32 columns x 32 rows x 1, no swizzle; reads outside [0,cols) x [0,T) are zero-filled
 int make_map_mn(CUtensorMap* map, const float* ptr, int cols, int T, int batches, long long ld, long long bstride) {
     EncodeTiledFn enc = encode_fn();
     B200_REQUIRE(enc != nullptr, "gemm: cuTensorMapEncodeTiled is not available from this driver");
     const cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)T, (cuuint64_t)batches};
     const cuuint64_t strides[2] = {(cuuint64_t)ld * sizeof(float), (cuuint64_t)(batches > 1 ? bstride : ld * (long long)T) * sizeof(float)};
-    const cuuint32_t box[3] = {32, (cuuint32_t)G_BK, 1};
+    const cuuint32_t box[3] = {32, (cuuint32_t)G_BK, 1};     // plain rows: the consumers transpose out of this image
     const cuuint32_t estr[3] = {1, 1, 1};
     const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), dims, strides, box, estr,
-                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     B200_REQUIRE(r == CUDA_SUCCESS, "gemm: cuTensorMapEncodeTiled failed (%d) for a [%d x %d x %d] operand", (int)r,
                  batches, T, cols);
@@ -438,9 +327,8 @@ int make_map_mn(CUtensorMap* map, const float* ptr, int cols, int T, int batches
 }
 
 // Split-K factor.  Few tiles (skinny products): one slice per idle SM.  A tile grid that is neither small nor a
-// multiple of the SM count (the recurrent weight gradients: 16 x 2 = 32 tiles x 4 slices = 128 CTAs on 148 SMs = 86 % of
-// the machine) is cut so that the CTA count lands just below a multiple of the SM count (32 x 9 = 288 CTAs = 1.95 waves =
-// 97 %) - as long as a slice keeps >= 64 K blocks and the partial tiles stay below 160 MB.
+// multiple of the SM count is cut so that the CTA count lands just below a multiple of the SM count - as long as a
+// slice keeps >= 64 K blocks and the partial tiles stay below 160 MB.
 int max_split(int M, int N) {
     const long long per = (long long)M * N * (long long)sizeof(float);
     long long s = (160LL << 20) / (per > 0 ? per : 1);
@@ -459,8 +347,6 @@ int pick_split(int M, int N, int KB) {
         const long long ctas = (long long)tiles * q;
         return (double)ctas / (double)(((ctas + sms - 1) / sms) * sms);
     };
-    // (measured: cutting a 128-tile grid 8 ways costs more in partial-tile traffic than the last 20 SMs bring - the
-    // kernel is close to the L2 feed rate there; for <= 74 tiles the finer cut wins: cfg B weight gradients 14.2 -> 13.5 ms)
     if (2 * tiles <= sms && eff(s) < 0.93) {
         const int cap = max_split(M, N);
         for (int q = s + 1; q <= cap && KB / q >= 64; ++q)
@@ -490,7 +376,7 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mb, GemmArgs g, void* ws, s
     nsplit = (g.KB + g.kb_per_split - 1) / g.kb_per_split;       // no empty slices
     g.partial = reinterpret_cast<float*>(ws);
     g.ch = gemm_chunk();
-    const size_t smem = (size_t)G_STAGES * G_STAGE_BYTES + 256;
+    const size_t smem = (size_t)GemmSmem<A_MN, B_MN>::STAGES * GemmSmem<A_MN, B_MN>::STAGE + 256;
     auto fn = gemm3x_kernel<A_MN, B_MN, B_PRE, A_PRE>;
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((g.N + G_BN - 1) / G_BN, (g.M + G_BM - 1) / G_BM, nsplit);
@@ -499,7 +385,7 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mb, GemmArgs g, void* ws, s
     if (nsplit > 1) {
         const long long total = (long long)g.M * g.N;
         int blocks = (int)((total + 255) / 256);
-        if (blocks > 2368) blocks = 2368;
+        if (blocks > 16 * sm_count()) blocks = 16 * sm_count();
         gemm3x_reduce_kernel<<<blocks, 256, 0, stream>>>(g.partial, nsplit, g.bias, g.C, g.M, g.N, g.ldc, g.accumulate,
                                                          g.perm);
         B200_LAUNCH_CHECK("gemm3x_reduce_kernel");
@@ -579,10 +465,8 @@ extern "C" int b200asr_gemm3x_tn_ws(const float* A, int lda, const float* B, con
 }
 
 static int gemm3x_nn_impl(const float* A, int lda, const float* B, int ldb, const float* bias, float* C, int M, int N,
-                          int K, int ldc, int accumulate, void* ws, size_t ws_bytes, b200asr_stream stream,
-                          const float* B_lo = nullptr, const float* A_lo = nullptr) {
+                          int K, int ldc, int accumulate, void* ws, size_t ws_bytes, b200asr_stream stream) {
     B200_REQUIRE(A && B && C, "gemm3x_nn: null pointer");
-    B200_REQUIRE(!A_lo || B_lo, "gemm3x_nn: a residual of A needs the residual of B as well");
     B200_REQUIRE(M > 0 && N > 0 && K > 0, "gemm3x_nn: bad sizes M=%d N=%d K=%d", M, N, K);
     B200_REQUIRE(lda >= K && (lda % 4) == 0 && ldb >= N && (ldb % 4) == 0 && ldc >= N,
                  "gemm3x_nn: row pitches must be multiples of 4 floats (lda %d ldb %d ldc %d)", lda, ldb, ldc);
@@ -595,20 +479,6 @@ static int gemm3x_nn_impl(const float* A, int lda, const float* B, int ldb, cons
     GemmArgs g = {};
     g.bias = bias; g.C = C; g.M = M; g.N = N; g.ldc = ldc; g.accumulate = accumulate;
     g.KB = (K + G_BK - 1) / G_BK; g.kbt = g.KB;
-    if (B_lo) {
-        B200_REQUIRE(aligned16(B_lo), "gemm3x_nn: operands must be 16-byte aligned");
-        CUtensorMap mlo;
-        rc = make_map_mn(&mlo, B_lo, N, K, 1, ldb, 0);
-        if (rc != B200_OK) return rc;
-        if (A_lo) {
-            B200_REQUIRE(aligned16(A_lo), "gemm3x_nn: operands must be 16-byte aligned");
-            CUtensorMap malo;
-            rc = make_map_k(&malo, A_lo, M, K, lda, G_BM);
-            if (rc != B200_OK) return rc;
-            return launch<false, true, true, true>(ma, mb, g, ws, ws_bytes, (cudaStream_t)stream, &mlo, &malo);
-        }
-        return launch<false, true, true>(ma, mb, g, ws, ws_bytes, (cudaStream_t)stream, &mlo);
-    }
     return launch<false, true>(ma, mb, g, ws, ws_bytes, (cudaStream_t)stream);
 }
 
@@ -623,12 +493,11 @@ extern "C" int b200asr_gemm3x_nn_ws(const float* A, int lda, const float* B, int
     return gemm3x_nn_impl(A, lda, B, ldb, bias, C, M, N, K, ldc, accumulate, workspace, workspace_bytes, stream);
 }
 
-static int gemm3x_nt_impl(const float* A, const float* A_lo, long long lda, long long a_bstride, int a_shift,
-                          const float* B, const float* B_lo, long long ldb, long long b_bstride, int b_shift, float* C,
-                          int M, int N, int T, int batches, int ldc, int accumulate, int permute_rows, void* workspace,
-                          size_t workspace_bytes, b200asr_stream stream) {
+extern "C" int b200asr_gemm3x_nt(const float* A, long long lda, long long a_bstride, int a_shift, const float* B,
+                                 long long ldb, long long b_bstride, int b_shift, float* C, int M, int N, int T,
+                                 int batches, int ldc, int accumulate, int permute_rows, void* workspace,
+                                 size_t workspace_bytes, b200asr_stream stream) {
     B200_REQUIRE(A && B && C, "gemm3x_nt: null pointer");
-    B200_REQUIRE(!A_lo || B_lo, "gemm3x_nt: a residual of A needs the residual of B as well");
     B200_REQUIRE(M > 0 && N > 0 && T > 0 && batches > 0, "gemm3x_nt: bad sizes M=%d N=%d T=%d batches=%d", M, N, T,
                  batches);
     // (a pitch smaller than the row length = overlapping rows: the in-place im2col view of a strided convolution)
@@ -647,35 +516,7 @@ static int gemm3x_nt_impl(const float* A, const float* A_lo, long long lda, long
     g.C = C; g.M = M; g.N = N; g.ldc = ldc; g.accumulate = accumulate; g.perm = permute_rows;
     g.kbt = (T + G_BK - 1) / G_BK; g.KB = g.kbt * batches;
     g.a_shift = a_shift; g.b_shift = b_shift;
-    if (B_lo) {
-        B200_REQUIRE(aligned16(B_lo) && (!A_lo || aligned16(A_lo)), "gemm3x_nt: operands must be 16-byte aligned");
-        CUtensorMap malo, mblo;
-        rc = make_map_mn(&mblo, B_lo, N, T, batches, ldb, b_bstride);
-        if (rc != B200_OK) return rc;
-        if (!A_lo)       // only the wide (256-column) operand pre-split: the splitters pass over the A tile alone
-            return launch<true, true, true, false>(ma, mb, g, workspace, workspace_bytes, (cudaStream_t)stream, &mblo);
-        rc = make_map_mn(&malo, A_lo, M, T, batches, lda, a_bstride);
-        if (rc != B200_OK) return rc;
-        return launch<true, true, true, true>(ma, mb, g, workspace, workspace_bytes, (cudaStream_t)stream, &mblo, &malo);
-    }
     return launch<true, true>(ma, mb, g, workspace, workspace_bytes, (cudaStream_t)stream);
-}
-
-extern "C" int b200asr_gemm3x_nt(const float* A, long long lda, long long a_bstride, int a_shift, const float* B,
-                                 long long ldb, long long b_bstride, int b_shift, float* C, int M, int N, int T,
-                                 int batches, int ldc, int accumulate, int permute_rows, void* workspace,
-                                 size_t workspace_bytes, b200asr_stream stream) {
-    return gemm3x_nt_impl(A, nullptr, lda, a_bstride, a_shift, B, nullptr, ldb, b_bstride, b_shift, C, M, N, T, batches, ldc,
-                          accumulate, permute_rows, workspace, workspace_bytes, stream);
-}
-
-extern "C" int b200asr_gemm3x_nt_pre(const float* A, const float* A_lo, long long lda, long long a_bstride, int a_shift,
-                                     const float* B, const float* B_lo, long long ldb, long long b_bstride, int b_shift,
-                                     float* C, int M, int N, int T, int batches, int ldc, int accumulate,
-                                     int permute_rows, void* workspace, size_t workspace_bytes, b200asr_stream stream) {
-    B200_REQUIRE(B_lo, "gemm3x_nt_pre: null residual of B (A_lo may be NULL: only B pre-split)");
-    return gemm3x_nt_impl(A, A_lo, lda, a_bstride, a_shift, B, B_lo, ldb, b_bstride, b_shift, C, M, N, T, batches, ldc,
-                          accumulate, permute_rows, workspace, workspace_bytes, stream);
 }
 
 extern "C" int b200asr_tf32_residual(const float* x, float* lo, long long n, b200asr_stream stream) {
@@ -694,13 +535,6 @@ extern "C" int b200asr_gemm3x_tn_pre(const float* A, int lda, const float* B, co
     return gemm3x_tn_impl(A, lda, B, bias, C, M, N, K, ldc, accumulate, workspace, workspace_bytes, stream, B_lo);
 }
 
-extern "C" int b200asr_gemm3x_nn_pre(const float* A, int lda, const float* B, const float* B_lo, int ldb, const float* bias,
-                                     float* C, int M, int N, int K, int ldc, int accumulate, void* workspace,
-                                     size_t workspace_bytes, b200asr_stream stream) {
-    B200_REQUIRE(B_lo, "gemm3x_nn_pre: null residual");
-    return gemm3x_nn_impl(A, lda, B, ldb, bias, C, M, N, K, ldc, accumulate, workspace, workspace_bytes, stream, B_lo);
-}
-
 extern "C" int b200asr_gemm3x_tn_pre2(const float* A, const float* A_lo, int lda, const float* B, const float* B_lo,
                                       const float* bias, float* C, int M, int N, int K, int ldc, int accumulate,
                                       void* workspace, size_t workspace_bytes, b200asr_stream stream) {
@@ -708,9 +542,3 @@ extern "C" int b200asr_gemm3x_tn_pre2(const float* A, const float* A_lo, int lda
     return gemm3x_tn_impl(A, lda, B, bias, C, M, N, K, ldc, accumulate, workspace, workspace_bytes, stream, B_lo, A_lo);
 }
 
-extern "C" int b200asr_gemm3x_nn_pre2(const float* A, const float* A_lo, int lda, const float* B, const float* B_lo, int ldb,
-                                      const float* bias, float* C, int M, int N, int K, int ldc, int accumulate,
-                                      void* workspace, size_t workspace_bytes, b200asr_stream stream) {
-    B200_REQUIRE(A_lo && B_lo, "gemm3x_nn_pre2: null residual");
-    return gemm3x_nn_impl(A, lda, B, ldb, bias, C, M, N, K, ldc, accumulate, workspace, workspace_bytes, stream, B_lo, A_lo);
-}

@@ -139,13 +139,14 @@ __device__ __forceinline__ void control_loop(const LstmParams& p, int T, unsigne
     }
 }
 
-// Packed fp32 FMA (Blackwell FFMA2): d.{lo,hi} = a.{lo,hi} * b + c.{lo,hi} with a scalar multiplier that ptxas
-// folds into the instruction's broadcast operand form - two FMAs per issue slot, which leaves issue bandwidth for
-// the shared-memory loads of the recurrence loops.
+// Pairs of fp32 FMAs on a packed register pair: d.{lo,hi} = a.{lo,hi} * b + c.{lo,hi} with a scalar multiplier.  Hopper
+// has no packed fp32 FMA instruction: the pair is two FFMAs (same rounding as the packed form).
 __device__ __forceinline__ unsigned long long ffma2_vs(unsigned long long a, float b, unsigned long long c) {
-    unsigned long long bb, d;
-    asm("mov.b64 %0, {%1, %1};" : "=l"(bb) : "f"(b));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(bb), "l"(c));
+    float alo, ahi, clo, chi;
+    unsigned long long d;
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(alo), "=f"(ahi) : "l"(a));
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(clo), "=f"(chi) : "l"(c));
+    asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(fmaf(alo, b, clo)), "f"(fmaf(ahi, b, chi)));
     return d;
 }
 __device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
@@ -215,8 +216,8 @@ __device__ __forceinline__ void fwd_group(const LstmParams& p, int g, int gt, in
 
         if (step > 0) {
             // Turn taking: the two groups of a CTA alternate on the FMA pipes (A, B, A, B, ...).  A group's loop runs
-            // ~1.6x faster alone than next to the other group's loop, and in strict alternation each group's state
-            // exchange (~5.6k cycles) is hidden behind the other group's loop instead of both groups waiting at once.
+            // faster alone than next to the other group's loop, and in strict alternation each group's state
+            // exchange is hidden behind the other group's loop instead of both groups waiting at once.
             if (p.NH == 2) {
                 if (g == 1) mbar_wait(&turn[1], (uint32_t)((step - 1) & 1));
                 else if (step >= 2) mbar_wait(&turn[0], (uint32_t)(step & 1));
@@ -738,7 +739,7 @@ __global__ void lstm_pack_mma_kernel(const float* __restrict__ w, float* __restr
 // ---- forward group, tensor cores: warp w of the group owns units [4w, 4w+4) of the CTA's unit block.
 // NS = number of k-step parities accumulated separately: a warp carries 6*NS independent MMA accumulator chains
 // (2 tiles x 3 products x NS); the dependent-issue latency of mma.sync is long enough that 6 chains leave the
-// tensor pipe idle (measured, tools/micro/mma_rate.cu).
+// tensor pipe idle.
 template <int NS>
 __device__ __forceinline__ void fwd_group_mma(const LstmParams& p, int g, int gt, int dir, int bg, int ub,
                                               const float4* Wm, const float* hsg, uint64_t* full, uint64_t* done,
@@ -1331,12 +1332,12 @@ struct Plan {
 };
 
 #ifndef LSTM_UMMA_BWD_DEFAULT
-#define LSTM_UMMA_BWD_DEFAULT 1     // validated on a B200 in round 2 (5.55 vs 8.02 us/step at B=64, H=512)
+#define LSTM_UMMA_BWD_DEFAULT 1
 #endif
 static int g_lstm_flags = 0;  // experiment switches, see LstmParams::flags (set through the upper bits of the mode)
-static int g_lstm_mode = 0;   // 0: tcgen05 (lstm_umma.cu) when the shape allows, else mma.sync, else fp32 FMA;
+static int g_lstm_mode = 0;   // 0: wgmma (lstm_umma.cu) when the shape allows, else mma.sync, else fp32 FMA;
                               // 1: always the fp32-FMA kernels, 2: mma.sync with 6 instead of 12 accumulator chains
-                              // (measurement only), 3: never tcgen05 (the mma.sync generation, for A/B comparisons)
+                              // (measurement only), 3: never wgmma (the mma.sync generation, for A/B comparisons)
 
 static int halves_for(int Bc) { return (Bc % 8 == 0) ? 2 : 1; }
 static int rows_for(int Bc) { return ((Bc / halves_for(Bc)) % 8 == 0) ? 8 : 4; }
@@ -1495,7 +1496,7 @@ static int bilstm_run(bool bwd, float* gates, const float* w_hh, float* cstate, 
     if (!bwd && g_lstm_mode == 0 && lstm_umma_fwd_supported(B, H, ndir))
         return lstm_umma_fwd(gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes,
                              (g_lstm_flags & 8) ? nullptr : g_trace, g_lstm_flags >> 4, stream);
-    // flag bit 5 (mode 512) toggles the backward between the tcgen05 kernel and the mma.sync generation
+    // flag bit 5 (mode 512) toggles the backward between the wgmma kernel and the mma.sync generation
     if (bwd && g_lstm_mode == 0 && (((g_lstm_flags & 32) != 0) != (LSTM_UMMA_BWD_DEFAULT != 0)) &&
         lstm_umma_bwd_supported(B, H, ndir, g_lstm_flags >> 4))
         return lstm_umma_bwd(gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes,

@@ -1,35 +1,34 @@
-// K7 on the 5th-generation tensor cores: the persistent BiLSTM recurrence with the step GEMM issued as tcgen05.mma
-// (kind::f16, fp32 accumulators in TMEM) instead of warp-level mma.sync.  Same CTA decomposition and the same
-// cross-SM exchange protocol as csrc/lstm.cu (one CTA per (direction, batch group of 32 rows, unit block), W_hh slice
-// resident in shared memory for all T steps, per-step release/acquire counter + 1-D bulk copies of the next state).
+// K7 on the Hopper tensor cores: the persistent BiLSTM recurrence with the step GEMM issued as warpgroup MMAs (wgmma,
+// f16 operands in shared memory, fp32 accumulators in registers) instead of warp-level mma.sync.  Same CTA
+// decomposition and the same cross-SM exchange protocol as csrc/lstm.cu (one CTA per (direction, batch group of 32
+// rows, unit block), W_hh slice resident in shared memory for all T steps, per-step release/acquire counter + 1-D bulk
+// copies of the next state).
 //
 // fp32 parity on a 16-bit tensor-core path - the "2 x 2 block" split product.  Every fp32 operand x is held as two
 // fp16 numbers  x = hi + lo / 2048,  hi = fp16(x),  lo = fp16((x - hi) * 2048)  (22+ significant bits; h in (-1,1) and
 // recurrent weights are far inside the fp16 range).  The step product h . W^T then needs hi.hi + (hi.lo + lo.hi)/2048.
-// Because a single CTA only has 32 batch rows and 4*UB <= 64 gate columns, one MMA has room to spare in M and N, so
-// the hi and lo parts are STACKED along M and N:
+// Because a single CTA only has 32 batch rows, the M = 64 of a warpgroup MMA has room to spare, so the hi and lo parts
+// are STACKED along M and N:
 //        A = [ h_hi ; h_lo ]  (M = 64 rows)        B = [ W_hi ; W_lo ]  (N = 8*UB rows),   both K-major over k = 0..H-1
-// and ONE tcgen05.mma per 16 values of k produces all four blocks hi.hi | hi.lo / lo.hi | lo.lo of D at the cost of a
-// single instruction (H/16 = 32 MMAs per step at H = 512 instead of 3 x 64 warp-level MMAs per warp).  The epilogue
-// adds  D[hi,hi] + (D[hi,lo] + D[lo,hi]) / 2048  (lo.lo is below fp32 resolution and dropped).
-// Row / column orders are chosen so that no shuffle or shared-memory round trip is needed after the TMEM load:
-//   A rows  : TMEM quadrant q (rows 16q..16q+15) = [hi of batch rows 8q..8q+7 ; lo of the same 8 rows]
-//   B rows  : n = 8g + 2*tq + e  <->  unit = 4*(g/2) + tq, gate = 2*(g%2) + e   (n < 4*UBp: hi, then the lo copy)
-//   tcgen05.ld.16x256b gives thread (r = lane/4, tq = lane%4) of a warp on quadrant q the hi row AND the lo row of
-//   batch row 8q+r at columns 8g + 2tq + {0,1}; the warp with unit quad j reads groups 2j and 2j+1 = all four gates
-//   of unit 4j + tq, for P1 = hi.hi, P2 = lo.hi and (second pair of loads) P3 = hi.lo: one LSTM cell per thread.
+// and one MMA per 16 values of k produces all four blocks hi.hi | hi.lo / lo.hi | lo.lo of D.  The epilogue adds
+// D[hi,hi] + (D[hi,lo] + D[lo,hi]) / 2048  (lo.lo is below fp32 resolution and dropped).
+// Row / column orders are chosen so that no shuffle or shared-memory round trip is needed after the MMA:
+//   A rows  : warp q of a warpgroup (rows 16q..16q+15) = [hi of batch rows 8q..8q+7 ; lo of the same 8 rows]
+//   B rows  : warpgroup j owns rows 32j..32j+31 = [hi | lo] x column groups (gates i,f | g,o) x (unit 4j + tq, gate e)
+//   so thread (r = lane/4, tq = lane%4) of warp q in warpgroup j receives, in its 16 accumulator registers, the hi row
+//   AND the lo row of batch row 8q+r for all four gates of unit 4j + tq, against W_hi and W_lo: one LSTM cell per thread.
 // The state exchange moves the next A operand between CTAs already in its shared-memory image (fp16 hi/lo, K-major,
 // 128-byte swizzle) and is pipelined per K ATOM (64 values of k = the hidden units of 64/UB producer CTAs): every
 // epilogue warp releases its stores with one red.release on the counter of the atom(s) its units belong to; lane a of
 // the consumer's control warp polls counter a and pulls atom a with one 8 KB bulk copy as soon as ITS producers are
-// done, and the MMA lane issues the four MMAs of an atom when it lands - the slowest producer, the copies and the MMAs
+// done, and the warpgroups issue the four MMAs of an atom when it lands - the slowest producer, the copies and the MMAs
 // of one step overlap instead of running back to back.  No CTA-wide barrier, fence or grid-wide counter in the loop.
 //
-// Reference behaviour restated: torch.nn.LSTM as called from /root/reference/src/module.py:112-113,129-132 (single
+// Reference behaviour restated: torch.nn.LSTM as called from the reference's src/module.py:112-113,129-132 (single
 // layer, batch_first, zero initial state, run over the zero-padded frames, gates i,f,g,o).
 #include <cuda_fp16.h>
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 #include "lstm_umma.h"
 
 namespace b200asr {
@@ -67,7 +66,7 @@ __device__ __forceinline__ void red_relaxed_add_u32(unsigned* p, unsigned v) {
 // consumer polls the flag with RELAXED gpu-scope loads (served at the L2 coherence point) and then only ISSUES A BULK
 // COPY, whose reads are performed by the TMA unit at L2 - this thread never reads the data through its own L1, and the
 // copy is control-dependent on the polled value.  `strict` adds the formal acquire (one more L2 round trip) and the
-// generic->async proxy fence of the PTX memory model (~1.4k cycles per step together); both variants are tested.
+// generic->async proxy fence of the PTX memory model; both variants are tested.
 __device__ __forceinline__ void ul_spin_until(const unsigned* ctr, unsigned target, int* err_flag, bool strict = false) {
     const long long t0 = clock64();
     while (ld_relaxed_u32(ctr) < target) {
@@ -94,7 +93,7 @@ constexpr int UL_NBUF = 8;
 #define UL_POLL_FWD_DEFAULT 0     // 1 once the polling exchange of the forward kernel is the validated default
 #endif
 #ifndef UL_POLL_BWD_DEFAULT
-#define UL_POLL_BWD_DEFAULT 1     // validated on a B200 in round 2 (5.14 vs 5.62 us/step at B=64, H=512)
+#define UL_POLL_BWD_DEFAULT 1
 #endif
 __device__ __forceinline__ uint4 ld_relaxed_v4(const void* p) {
     uint4 v;
@@ -157,7 +156,8 @@ __global__ void ul_pack_fwd_kernel(const float* __restrict__ w, uint8_t* __restr
         __half hi, lo;
         split_f16(v, hi, lo);
         uint8_t* img = dst + (size_t)cta * ((size_t)NA * N * 128);
-        const uint32_t off = (uint32_t)(k >> 6) * (N * 128) + umma::sw128_offset(n, (k & 63) * 2);
+        const int row = 32 * (g >> 1) + (n < NH ? 0 : 16) + 8 * (g & 1) + (nn & 7);   // warpgroup g/2: [hi | lo] x (if | go)
+        const uint32_t off = (uint32_t)(k >> 6) * (N * 128) + wgmma::sw128_offset(row, (k & 63) * 2);
         *reinterpret_cast<__half*>(img + off) = (n < NH) ? hi : lo;
     }
 }
@@ -165,27 +165,22 @@ __global__ void ul_pack_fwd_kernel(const float* __restrict__ w, uint8_t* __restr
 #define UL_TRACE(slot) \
     do { if (p.trace && blockIdx.x == 0) p.trace[(size_t)step * 16 + (slot)] = clock64(); } while (0)
 
-// Warp roles: warps [0, UBP) epilogue / pointwise - warp w owns TMEM quadrant q = w % 4 (the hardware rule) and the
-// unit quad j = w / 4, i.e. ONE cell (batch row 8q + lane/4, unit 4j + lane%4) per thread; warp UBP = MMA issue (one
-// lane) and TMEM allocation; warp UBP+1 = publisher (one lane: ONE gpu-scope fence + release per CTA and step, after
-// the epilogue warps arrived on `pub`); warps UBP+2 .. UBP+1+NC = control, one lane each, control warp c owns K atoms
-// c, c+NC, ...
+// Warp roles: warps [0, UBP) MMA + epilogue / pointwise - UBP/4 warpgroups; warp w is warp q = w % 4 of warpgroup
+// j = w / 4 (the unit quad), i.e. ONE cell (batch row 8q + lane/4, unit 4j + lane%4) per thread; warp UBP = publisher
+// (one lane: ONE gpu-scope fence + release per CTA and step, after the epilogue warps arrived on `pub`); warps
+// UBP+1 .. UBP+NC = control, one lane each, control warp c owns K atoms c, c+NC, ...
 template <int UBP, bool POLL>
-__global__ void __launch_bounds__(32 * (UBP + 2 + UL_MAX_CTRL), 1) bilstm_fwd_umma_kernel(UlParams p) {
+__global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_umma_kernel(UlParams p) {
     constexpr int N = 8 * UBP;            // B operand rows (gate columns, hi + lo copies)
-    constexpr int NH = 4 * UBP;
-    constexpr uint32_t TMEM_COLS = N <= 32 ? 32 : N <= 64 ? 64 : N <= 128 ? 128 : 256;
     extern __shared__ __align__(1024) uint8_t smem[];
     const int H = p.H, T = p.T, NA = p.NA, UB = p.UB;
     uint8_t* sA = smem;
     uint8_t* sB = smem + (size_t)NA * UL_ATOM_A;
     uint64_t* full = reinterpret_cast<uint64_t*>(sB + (size_t)NA * N * 128);    // [UL_MAX_ATOMS]
-    uint64_t* d_free = full + UL_MAX_ATOMS;      // the epilogue warps have read D out of TMEM
-    uint64_t* mma_done = d_free + 1;
-    uint64_t* wload = d_free + 2;
-    uint64_t* pub = d_free + 3;                  // the epilogue warps have stored h_step
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(d_free + 4);
-    uint64_t* landed = d_free + 5;               // [UL_MAX_ATOMS] polling exchange: a bulk copy of the atom has landed
+    uint64_t* mma_done = full + UL_MAX_ATOMS;    // the MMAs of a step have read every atom of A (one arrival per warp)
+    uint64_t* wload = mma_done + 1;
+    uint64_t* pub = mma_done + 2;                // the epilogue warps have stored h_step
+    uint64_t* landed = mma_done + 3;             // [UL_MAX_ATOMS] polling exchange: a bulk copy of the atom has landed
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int NC = p.NC;
@@ -199,24 +194,19 @@ __global__ void __launch_bounds__(32 * (UBP + 2 + UL_MAX_CTRL), 1) bilstm_fwd_um
             mbar_init(&full[a], 1);
             mbar_init(&landed[a], 1);
         }
-        mbar_init(d_free, UBP);
         mbar_init(pub, UBP);
-        mbar_init(mma_done, 1);
+        mbar_init(mma_done, UBP);
         mbar_init(wload, 1);
         mbar_fence_init();
     }
-    if (warp == UBP) umma::tmem_alloc(tmem_slot, TMEM_COLS);
-    umma::fence_before_sync();
     __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem = *tmem_slot;
     const size_t img_bytes = (size_t)NA * UL_ATOM_A;             // one image of the A operand
     uint8_t* xb = p.xbuf + ((size_t)dir * p.nbg + bg) * (POLL ? UL_NBUF : 2) * img_bytes;
     unsigned* ctr0 = p.counters + ((size_t)dir * p.nbg + bg) * UL_MAX_ATOMS;
 
-    if (POLL && warp > UBP) {
-        // ------------------------------------------------------------------ loader warps (warp UBP+1 loads W first)
-        const int c = warp - UBP - 1;                 // 0 .. UL_MAX_CTRL
+    if (POLL && warp >= UBP) {
+        // ------------------------------------------------------------------ loader warps (warp UBP only loads W)
+        const int c = warp - UBP;                     // 0 .. UL_MAX_CTRL
         if (c == 0) {
             if (lane == 0) {
                 const uint8_t* wsrc = p.wpack + ((size_t)dir * p.nub + ub) * ((size_t)NA * N * 128);
@@ -271,7 +261,7 @@ __global__ void __launch_bounds__(32 * (UBP + 2 + UL_MAX_CTRL), 1) bilstm_fwd_um
                 }
             }
         }
-    } else if (warp == UBP + 1) {
+    } else if (warp == UBP) {
         // ------------------------------------------------------------------ publisher lane
         if (lane == 0) {
             const int a0 = (ub * UB) >> 6, a1 = (ub * UB + UB - 1) >> 6;
@@ -284,9 +274,9 @@ __global__ void __launch_bounds__(32 * (UBP + 2 + UL_MAX_CTRL), 1) bilstm_fwd_um
                 UL_TRACE(9);
             }
         }
-    } else if (warp > UBP + 1) {
+    } else if (warp > UBP) {
         // ------------------------------------------------------------------ control warps (one lane each)
-        const int c = warp - UBP - 2;
+        const int c = warp - UBP - 1;
         if (lane == 0 && c < NC) {
             if (c == 0) {
                 const uint8_t* wsrc = p.wpack + ((size_t)dir * p.nub + ub) * ((size_t)NA * N * 128);
@@ -316,42 +306,18 @@ __global__ void __launch_bounds__(32 * (UBP + 2 + UL_MAX_CTRL), 1) bilstm_fwd_um
                 }
             }
         }
-    } else if (warp == UBP) {
-        // ------------------------------------------------------------------ MMA lane
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma::instr_desc(umma::FMT_F16, 64, N);
-            const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
-            mbar_wait(wload, 0);
-            for (int step = 1; step < T; ++step) {
-                if (step > 1) mbar_wait(d_free, (uint32_t)(step & 1));      // epilogue of step-1 has drained D
-                for (int a = 0; a < NA; ++a) {
-                    mbar_wait(&full[a], (uint32_t)((step - 1) & 1));
-                    umma::fence_after_sync();
-                    if (a == 0) UL_TRACE(1);
-                    if (a == NA - 1) UL_TRACE(6);
-                    if (a == NA / 2) UL_TRACE(14);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const uint64_t da = umma::desc_k_sw128(a_base + a * UL_ATOM_A + j * 32);
-                        const uint64_t db = umma::desc_k_sw128(b_base + a * (N * 128) + j * 32);
-                        umma::mma_ss<umma::FMT_F16>(tmem, da, db, idesc, (a | j) != 0);
-                    }
-                }
-                umma::commit(mma_done);
-                UL_TRACE(2);
-            }
-        }
     } else {
-        // ------------------------------------------------------------------ epilogue / pointwise warps
+        // ------------------------------------------------------------------ MMA + epilogue / pointwise warps
         const int q = warp & 3, jq = warp >> 2, r = lane >> 2, tq = lane & 3;
         const int brow = p.b0 + bg * UL_BC + 8 * q + r;
         const int unit = 4 * jq + tq;                     // my unit of the CTA's block
         const bool ok = (brow < p.Bend) && (unit < UB);
         const int ug = ub * UB + (unit < UB ? unit : 0);  // = my k in the next A operand
-        const uint32_t t_lane = tmem + ((uint32_t)(32 * q) << 16);
+        const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB) + jq * (32 * 128);
+        float d[16];
         const int a_row_hi = 16 * q + r, a_row_lo = 16 * q + 8 + r;
-        const uint32_t pub_hi = (uint32_t)(ug >> 6) * UL_ATOM_A + umma::sw128_offset(a_row_hi, (ug & 63) * 2);
-        const uint32_t pub_lo = (uint32_t)(ug >> 6) * UL_ATOM_A + umma::sw128_offset(a_row_lo, (ug & 63) * 2);
+        const uint32_t pub_hi = (uint32_t)(ug >> 6) * UL_ATOM_A + wgmma::sw128_offset(a_row_hi, (ug & 63) * 2);
+        const uint32_t pub_lo = (uint32_t)(ug >> 6) * UL_ATOM_A + wgmma::sw128_offset(a_row_lo, (ug & 63) * 2);
         float c_reg = 0.f;
         const bool trc = (warp == 0 && lane == 0);
         float4 st_g = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -366,19 +332,27 @@ __global__ void __launch_bounds__(32 * (UBP + 2 + UL_MAX_CTRL), 1) bilstm_fwd_um
             float4 pre = make_float4(0.f, 0.f, 0.f, 0.f);
             if (ok) pre = *reinterpret_cast<const float4*>(p.gates + (rowbase * H + ug) * 4);
             if (step > 0) {
-                mbar_wait(mma_done, (uint32_t)((step - 1) & 1));
-                umma::fence_after_sync();
-                if (trc) UL_TRACE(3);
-                // column group g = 2*jq + gh holds gates (2gh, 2gh+1) of my unit: v0,v1 = hi row, v2,v3 = lo row
-                uint32_t dif[4], dgo[4], eif[4], ego[4];
-                umma::ld_16x256b_x1(t_lane + 16 * jq, dif);
-                umma::ld_16x256b_x1(t_lane + 16 * jq + 8, dgo);
-                umma::ld_16x256b_x1(t_lane + NH + 16 * jq, eif);
-                umma::ld_16x256b_x1(t_lane + NH + 16 * jq + 8, ego);
-                umma::wait_ld();
-                umma::fence_before_sync();      // my TMEM reads are done: the next step's MMAs may overwrite D
+                if (step == 1) mbar_wait(wload, 0);
+                wgmma::fence_operand(d);
+                wgmma::fence();
+                for (int a = 0; a < NA; ++a) {
+                    mbar_wait(&full[a], (uint32_t)((step - 1) & 1));
+                    if (trc && a == 0) UL_TRACE(1);
+                    if (trc && a == NA - 1) UL_TRACE(6);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j)
+                        wgmma::mma_f16_n32(d, wgmma::desc_k_sw128(a_base + a * UL_ATOM_A + j * 32),
+                                           wgmma::desc_k_sw128(b_base + a * (N * 128) + j * 32), (a | j) != 0);
+                }
+                wgmma::commit_group();
+                if (trc) UL_TRACE(2);
+                wgmma::wait_all();
+                wgmma::fence_operand(d);
                 __syncwarp();
-                if (lane == 0) ul_arrive(d_free);
+                if (lane == 0) ul_arrive(mma_done);     // the control warps may overwrite the atoms of A
+                if (trc) UL_TRACE(3);
+                // d[0..7]: hi and lo row against W_hi, gates (i,f) then (g,o); d[8..15]: the same against W_lo
+                const float *dif = d, *dgo = d + 4, *eif = d + 8, *ego = d + 12;
                 if (trc) UL_TRACE(4);
                 if (st_pending) {
                     *reinterpret_cast<float4*>(p.gates + (st_row * H + ug) * 4) = st_g;
@@ -387,10 +361,10 @@ __global__ void __launch_bounds__(32 * (UBP + 2 + UL_MAX_CTRL), 1) bilstm_fwd_um
                     st_pending = false;
                 }
                 const float k = 1.f / 2048.f;
-                pre.x += __uint_as_float(dif[0]) + (__uint_as_float(dif[2]) + __uint_as_float(eif[0])) * k;
-                pre.y += __uint_as_float(dif[1]) + (__uint_as_float(dif[3]) + __uint_as_float(eif[1])) * k;
-                pre.z += __uint_as_float(dgo[0]) + (__uint_as_float(dgo[2]) + __uint_as_float(ego[0])) * k;
-                pre.w += __uint_as_float(dgo[1]) + (__uint_as_float(dgo[3]) + __uint_as_float(ego[1])) * k;
+                pre.x += dif[0] + (dif[2] + eif[0]) * k;
+                pre.y += dif[1] + (dif[3] + eif[1]) * k;
+                pre.z += dgo[0] + (dgo[2] + ego[0]) * k;
+                pre.w += dgo[1] + (dgo[3] + ego[1]) * k;
             }
             const float ig = sigmoidf_(pre.x);
             const float fg = sigmoidf_(pre.y);
@@ -452,7 +426,7 @@ __global__ void __launch_bounds__(32 * (UBP + 2 + UL_MAX_CTRL), 1) bilstm_fwd_um
                 }
                 if (trc) UL_TRACE(5);
             }
-            // the stash / output stores of this step are issued during the NEXT step (after its TMEM loads): stores
+            // the stash / output stores of this step are issued during the NEXT step (after its MMAs): stores
             // in flight while the publisher runs its gpu-scope fence lengthen that fence by their L2 round trip
             st_g = make_float4(ig, fg, gg, og);
             st_c = c;
@@ -467,23 +441,21 @@ __global__ void __launch_bounds__(32 * (UBP + 2 + UL_MAX_CTRL), 1) bilstm_fwd_um
             p.out[st_out] = st_h;
         }
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == UBP) umma::tmem_dealloc(tmem, TMEM_COLS);
 }
 
 // =====================================================================================================================
-// Backward (BPTT) step on tcgen05.  Per CTA (direction, batch group of 32 rows, unit block of UB units) and step:
+// Backward (BPTT) step on wgmma.  Per CTA (direction, batch group of 32 rows, unit block of UB units) and step:
 //   dh = dOut[b,t] + sum_src partial_src[b, my units]          (inbox: one [32 x UB] fp32 block per source CTA)
 //   pointwise -> dG[b, 4*UB] (written to the gate stash in place), dc carried in a register
 //   partial_me[b, 0..H) = dG[32 x 4UB] . W_slice[4UB x H]      -> scattered to every destination CTA's inbox
 // The step GEMM has K = 4*UB <= 64 (ONE 128-byte K atom) and N = H, so the tensor core is fed with
-//   A1 = [ dG_hi ; dG_lo ]  and  A2 = [ 0 ; dG_hi ]   (M = 64: per TMEM quadrant 8 "hi" rows then 8 "lo" rows)
+//   A1 = [ dG_hi ; dG_lo ]  and  A2 = [ 0 ; dG_hi ]   (M = 64: per warp 8 "hi" rows then 8 "lo" rows)
 //   D[:, n-block] = A1 . W_hi^T + A2 . W_lo^T
-// i.e. the hi rows of D hold dG_hi.W_hi and the lo rows hold dG_lo.W_hi + dG_hi.W_lo (both scaled by 2048): ONE
-// accumulator region of 512 columns, 2*(4UB/16) MMAs of N = 256 per n-block, and tcgen05.ld.16x256b hands every
-// drain thread the (hi, lo) pair of the same (row, column).  dG has no bounded range, so every batch row is scaled by
-// a power of two that brings its largest |dG| to [2^13, 2^14) before the fp16 hi/lo split; the drain undoes it.
+// i.e. the hi rows of D hold dG_hi.W_hi and the lo rows hold dG_lo.W_hi + dG_hi.W_lo (both scaled by 2048); of every
+// 256 columns, warpgroup jq accumulates columns 64jq .. 64jq+63 (2*(4UB/16) MMAs of N = 64), and the accumulator
+// fragment hands every thread the (hi, lo) pair of the same (row, column).  dG has no bounded range, so every batch
+// row is scaled by a power of two that brings its largest |dG| to [2^13, 2^14) before the fp16 hi/lo split; the drain
+// undoes it.
 template <int UB>
 __global__ void ul_pack_bwd_kernel(const float* __restrict__ w, uint8_t* __restrict__ dst, int H, int ndir) {
     const int nub = H / UB;
@@ -502,7 +474,7 @@ __global__ void ul_pack_bwd_kernel(const float* __restrict__ w, uint8_t* __restr
         __half hi, lo;
         split_f16(v, hi, lo);
         uint8_t* img = dst + (size_t)cta * ((size_t)2 * H * 128) + (size_t)part * H * 128;
-        *reinterpret_cast<__half*>(img + umma::sw128_offset(n, k * 2)) = part ? lo : hi;
+        *reinterpret_cast<__half*>(img + wgmma::sw128_offset(n, k * 2)) = part ? lo : hi;
     }
 }
 
@@ -515,15 +487,11 @@ constexpr int ULB_CTRL = 4;
 // destination polls its inbox IN GLOBAL MEMORY (L2) with relaxed loads until every word shows the expected tag and sums
 // straight from registers: no fence, no counter, no bulk copy, no shared-memory inbox.
 template <int UB, bool POLL>
-__global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 2 + ULB_CTRL), 1) bilstm_bwd_umma_kernel(UlParams p) {
+__global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm_bwd_umma_kernel(UlParams p) {
     constexpr int KS = (4 * UB) / 16;               // MMAs (k-steps of 16) per product and n-block
     extern __shared__ __align__(1024) uint8_t smem[];
     const int H = p.H, T = p.T, nub = p.nub;
-    // n-blocks of (up to) 256 accumulator columns; they alternate over TWO 256-column TMEM buffers, so H = 640 (cfg D:
-    // 256 + 256 + 128) fits the 512 columns: block 2 re-uses buffer 0 once block 0 of the same step has been drained.
-    // Barrier phases count the USES of a buffer: use(j, step) = step * uses_per_step[j & 1] + j / 2.
-    const int NB = (H + 255) / 256;
-    const int ups0 = (NB + 1) / 2, ups1 = NB / 2;
+    const int NB = (H + 255) / 256;                 // n-blocks of (up to) 256 columns, 64 per warpgroup
     uint8_t* sWhi = smem;
     uint8_t* sWlo = smem + (size_t)H * 128;
     uint8_t* sA1 = sWlo + (size_t)H * 128;
@@ -533,49 +501,39 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 2 + ULB_CTRL), 1) bilstm
     float* rscale = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(inbox) + inbox_bytes);   // [32]
     uint64_t* in_full = reinterpret_cast<uint64_t*>(rscale + 32);
     uint64_t* a_ready = in_full + 1;
-    uint64_t* mma_done = in_full + 2;               // [2]
-    uint64_t* d_free = in_full + 4;                 // [2]
-    uint64_t* pub = in_full + 6;
-    uint64_t* wload = in_full + 7;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(in_full + 8);
+    uint64_t* mma_done = in_full + 2;               // the MMAs of a step have read the A tiles (one arrival per warp)
+    uint64_t* pub = in_full + 3;
+    uint64_t* wload = in_full + 4;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     int blk = blockIdx.x;
     const int ub = blk % p.nub; blk /= p.nub;
     const int bg = blk % p.nbg; blk /= p.nbg;
     const int dir = blk;
-    const uint32_t tmem_cols = H <= 256 ? 256u : 512u;
 
     for (int i = tid; i < 16384 / 16; i += blockDim.x) reinterpret_cast<uint4*>(sA1)[i] = make_uint4(0, 0, 0, 0);
     if (tid == 0) {
         mbar_init(in_full, ULB_CTRL);
         mbar_init(a_ready, ULB_EPI_WARPS);
-        for (int j = 0; j < 2; ++j) {
-            mbar_init(&mma_done[j], 1);
-            mbar_init(&d_free[j], ULB_EPI_WARPS);
-        }
+        mbar_init(mma_done, ULB_EPI_WARPS);
         mbar_init(pub, ULB_EPI_WARPS);
         mbar_init(wload, 1);
         mbar_fence_init();
     }
-    if (warp == ULB_EPI_WARPS) umma::tmem_alloc(tmem_slot, tmem_cols);
     fence_proxy_async_smem();
-    umma::fence_before_sync();
     __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem = *tmem_slot;
     const size_t xelems = (size_t)nub * nub * UL_BC * UB;                       // one parity buffer of one (dir, bg)
     float* xb = reinterpret_cast<float*>(p.xbuf) + ((size_t)dir * p.nbg + bg) * 2 * xelems;
     unsigned* ctr = p.counters + ((size_t)dir * p.nbg + bg);
 
-    if (POLL && warp > ULB_EPI_WARPS) {
-        if (warp == ULB_EPI_WARPS + 2 && lane == 0) {            // only the W load is left for the control warps
+    if (POLL && warp >= ULB_EPI_WARPS) {
+        if (warp == ULB_EPI_WARPS + 1 && lane == 0) {            // only the W load is left for the control warps
             const uint8_t* wsrc = p.wpack + ((size_t)dir * p.nub + ub) * ((size_t)2 * H * 128);
             mbar_expect_tx(wload, (uint32_t)(2 * H * 128));
             for (int off = 0; off < 2 * H * 128; off += 32768)
                 bulk_g2s(sWhi + off, wsrc + off, 32768, wload);
         }
-    } else if (warp == ULB_EPI_WARPS + 1) {
+    } else if (warp == ULB_EPI_WARPS) {
         // ------------------------------------------------------------------ publisher lane
         if (lane == 0) {
             for (int step = 0; step + 1 < T; ++step) {
@@ -586,9 +544,9 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 2 + ULB_CTRL), 1) bilstm
                 UL_TRACE(9);
             }
         }
-    } else if (warp > ULB_EPI_WARPS + 1) {
+    } else if (warp > ULB_EPI_WARPS) {
         // ------------------------------------------------------------------ control lanes: W load, inbox pulls
-        const int c = warp - ULB_EPI_WARPS - 2;
+        const int c = warp - ULB_EPI_WARPS - 1;
         if (lane == 0) {
             if (c == 0) {
                 const uint8_t* wsrc = p.wpack + ((size_t)dir * p.nub + ub) * ((size_t)2 * H * 128);
@@ -599,10 +557,7 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 2 + ULB_CTRL), 1) bilstm
             const uint32_t chunk = (uint32_t)(inbox_bytes / ULB_CTRL);
             for (int step = 0; step + 1 < T; ++step) {
                 // my epilogue warps summed the inbox of `step` before they released the A tile of `step`
-                {
-                    const int jl = NB - 1, ul = step * ((jl & 1) ? ups1 : ups0) + (jl >> 1);
-                    mbar_wait(&mma_done[jl & 1], (uint32_t)(ul & 1));
-                }
+                mbar_wait(mma_done, (uint32_t)(step & 1));
                 ul_spin_until(ctr, (unsigned)(step + 1) * (unsigned)nub, p.err_flag, (p.flags & 1) != 0);
                 if (c == 0) UL_TRACE(10);
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(xb + (size_t)(step & 1) * xelems +
@@ -612,35 +567,8 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 2 + ULB_CTRL), 1) bilstm
                 if (c == 0) UL_TRACE(11);
             }
         }
-    } else if (warp == ULB_EPI_WARPS) {
-        // ------------------------------------------------------------------ MMA lane
-        if (lane == 0) {
-            const uint32_t a1 = smem_u32(sA1), a2 = smem_u32(sA2), whi = smem_u32(sWhi), wlo = smem_u32(sWlo);
-            mbar_wait(wload, 0);
-            for (int step = 0; step + 1 < T; ++step) {
-                mbar_wait(a_ready, (uint32_t)(step & 1));
-                umma::fence_after_sync();
-                UL_TRACE(1);
-                for (int j = 0; j < NB; ++j) {
-                    const int buf = j & 1, use = step * (buf ? ups1 : ups0) + (j >> 1);
-                    if (use > 0) mbar_wait(&d_free[buf], (uint32_t)((use - 1) & 1));   // previous use has been drained
-                    umma::fence_after_sync();
-                    const int ncols = min(256, H - 256 * j);
-                    const uint32_t idesc = umma::instr_desc(umma::FMT_F16, 64, ncols);
-#pragma unroll
-                    for (int kk = 0; kk < KS; ++kk) {
-                        umma::mma_ss<umma::FMT_F16>(tmem + 256 * buf, umma::desc_k_sw128(a1 + kk * 32),
-                                                    umma::desc_k_sw128(whi + j * 32768 + kk * 32), idesc, kk > 0);
-                        umma::mma_ss<umma::FMT_F16>(tmem + 256 * buf, umma::desc_k_sw128(a2 + kk * 32),
-                                                    umma::desc_k_sw128(wlo + j * 32768 + kk * 32), idesc, 1);
-                    }
-                    umma::commit(&mma_done[buf]);
-                }
-                UL_TRACE(2);
-            }
-        }
     } else {
-        // ------------------------------------------------------------------ pointwise + drain warps
+        // ------------------------------------------------------------------ pointwise + MMA + drain warps
         // pointwise mapping: cell i = warp*32 + lane -> (batch row b = i / UB, unit u = i % UB)
         const int ci = warp * 32 + lane;
         const bool cell = ci < UL_BC * UB;
@@ -649,11 +577,12 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 2 + ULB_CTRL), 1) bilstm
         const bool ok = cell && brow < p.Bend;
         const int ug = ub * UB + u;
         const int row_hi = 16 * (b >> 3) + (b & 7), row_lo = row_hi + 8;
-        const uint32_t off_hi = umma::sw128_offset(row_hi, 8 * u), off_lo = umma::sw128_offset(row_lo, 8 * u);
-        // drain mapping: TMEM quadrant q, column quarter jq of every n-block
+        const uint32_t off_hi = wgmma::sw128_offset(row_hi, 8 * u), off_lo = wgmma::sw128_offset(row_lo, 8 * u);
+        // MMA / drain mapping: warp q of warpgroup jq = column quarter jq of every n-block
         const int q = warp & 3, jq = warp >> 2, r = lane >> 2, tq = lane & 3;
         const int drow = 8 * q + r;
-        const uint32_t t_lane = tmem + ((uint32_t)(32 * q) << 16);
+        const uint32_t a1 = smem_u32(sA1), a2 = smem_u32(sA2), whi = smem_u32(sWhi), wlo = smem_u32(sWlo);
+        float d[32];
         float dc_reg = 0.f;
         const bool trc = (warp == 0 && lane == 0);
 
@@ -751,6 +680,8 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 2 + ULB_CTRL), 1) bilstm
                 int e = (int)((__float_as_uint(m) >> 23) & 0xffu) - 127;
                 e = e < -100 ? -100 : (e > 100 ? 100 : e);
                 const float sc = __uint_as_float((uint32_t)(127 + 13 - e) << 23);
+                // every warpgroup's MMAs of the previous step have read the A tiles (and the drains the row scales)
+                if (step > 0) mbar_wait(mma_done, (uint32_t)((step - 1) & 1));
                 if (cell) {
                     if (u == 0) rscale[b] = __uint_as_float((uint32_t)(127 + e - 13) << 23);
                     __half hi[4], lo[4];
@@ -770,37 +701,38 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 2 + ULB_CTRL), 1) bilstm
                 __syncwarp();
                 if (lane == 0) ul_arrive(a_ready);
                 if (trc) UL_TRACE(5);
-                // ---- drain the accumulator into the destinations' inboxes, n-block by n-block
+                if (step == 0) mbar_wait(wload, 0);
+                mbar_wait(a_ready, (uint32_t)(step & 1));           // all 16 warps wrote (and fenced) their part of A
+                if (trc) UL_TRACE(1);
+                // ---- MMA + drain of the accumulator into the destinations' inboxes, n-block by n-block
                 float* outbase = xb + (size_t)(step & 1) * xelems;
                 for (int j = 0; j < NB; ++j) {
-                    const int buf = j & 1, use = step * (buf ? ups1 : ups0) + (j >> 1);
-                    const bool mine = 256 * j + 64 * jq < H;          // the last block of H = 640 is only 128 wide
-                    if (!mine) {                                      // nothing of this block is mine: just release it
-                        __syncwarp();
-                        if (lane == 0) ul_arrive(&d_free[buf]);
-                        continue;
+                    if (256 * j + 64 * jq >= H) continue;             // the last block of H = 640 is only 128 wide
+                    const uint32_t boff = (uint32_t)(256 * j + 64 * jq) * 128u;
+                    wgmma::fence_operand(d);
+                    wgmma::fence();
+#pragma unroll
+                    for (int kk = 0; kk < KS; ++kk) {
+                        wgmma::mma_f16_n64(d, wgmma::desc_k_sw128(a1 + kk * 32), wgmma::desc_k_sw128(whi + boff + kk * 32), kk > 0);
+                        wgmma::mma_f16_n64(d, wgmma::desc_k_sw128(a2 + kk * 32), wgmma::desc_k_sw128(wlo + boff + kk * 32), 1);
                     }
-                    mbar_wait(&mma_done[buf], (uint32_t)(use & 1));
-                    umma::fence_after_sync();
+                    wgmma::commit_group();
+                    wgmma::wait_all();
+                    wgmma::fence_operand(d);
                     if (trc && j == 0) UL_TRACE(6);
-                    uint32_t v0[16], v1[16];
-                    umma::ld_16x256b_x4(t_lane + 256 * buf + 64 * jq, v0);
-                    umma::ld_16x256b_x4(t_lane + 256 * buf + 64 * jq + 32, v1);
-                    umma::wait_ld();
-                    umma::fence_before_sync();
-                    __syncwarp();
-                    if (lane == 0) ul_arrive(&d_free[buf]);
+                    const float* v0 = d;
+                    const float* v1 = d + 16;
                     const float rs = rscale[drow];
                     const float k = 1.f / 2048.f;
 #pragma unroll
                     for (int hh = 0; hh < 2; ++hh) {
 #pragma unroll
                         for (int g = 0; g < 4; ++g) {
-                            const uint32_t* v = hh ? &v1[4 * g] : &v0[4 * g];
+                            const float* v = hh ? &v1[4 * g] : &v0[4 * g];
                             const int n = 256 * j + 64 * jq + 32 * hh + 8 * g + 2 * tq;
                             const int dst = n / UB, uu = n - dst * UB;
-                            const float o0 = (__uint_as_float(v[0]) + __uint_as_float(v[2]) * k) * rs;
-                            const float o1 = (__uint_as_float(v[1]) + __uint_as_float(v[3]) * k) * rs;
+                            const float o0 = (v[0] + v[2] * k) * rs;
+                            const float o1 = (v[1] + v[3] * k) * rs;
                             float* optr = outbase + (((size_t)dst * nub + ub) * UL_BC + drow) * UB + uu;
                             if (POLL) {
                                 const uint32_t tagw = (uint32_t)((step >> 1) & 1) ^ 1u;
@@ -811,17 +743,15 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 2 + ULB_CTRL), 1) bilstm
                         }
                     }
                 }
-                if (!POLL) {
-                    __syncwarp();
-                    if (lane == 0) ul_arrive(pub);
+                __syncwarp();
+                if (lane == 0) {
+                    ul_arrive(mma_done);
+                    if (!POLL) ul_arrive(pub);
                 }
                 if (trc) UL_TRACE(7);
             }
         }
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == ULB_EPI_WARPS) umma::tmem_dealloc(tmem, tmem_cols);
 }
 
 struct UlPlan {
@@ -872,7 +802,7 @@ int ul_launch_fwd(const UlPlan& pl, UlParams p, const float* w_hh, cudaStream_t 
     const void* fn = (const void*)bilstm_fwd_umma_kernel<UBP, POLL>;
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
     int per_sm = 0;
-    const int threads = 32 * (UBP + 2 + p.NC);
+    const int threads = 32 * (UBP + 1 + p.NC);
     B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, pl.smem));
     B200_REQUIRE((long long)per_sm * sm_count() >= pl.ctas, "bilstm(umma): %d CTAs cannot be co-resident (%d/SM x %d SMs)",
                  pl.ctas, per_sm, sm_count());
@@ -894,7 +824,7 @@ struct UlbPlan {
 };
 
 int ulb_plan(int B, int H, int ndir, bool poll, UlbPlan* out) {
-    // accumulator = H columns in n-blocks of 256 over two TMEM buffers: 256 | 512 | 640 | 768 (a last block of 128 or 256)
+    // accumulator = H columns in n-blocks of 256, 64 per warpgroup: 256 | 512 | 640 | 768 (a last block of 128 or 256)
     if (H % 128 != 0 || H < 256 || H > 768) return -1;
     const int sms = sm_count();
     const size_t cap = (size_t)max_optin_smem();
@@ -934,7 +864,7 @@ int ul_launch_bwd(const UlbPlan& pl, UlParams p, const float* w_hh, cudaStream_t
     const void* fn = (const void*)bilstm_bwd_umma_kernel<UB, POLL>;
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
     int per_sm = 0;
-    const int threads = 32 * (ULB_EPI_WARPS + 2 + ULB_CTRL);
+    const int threads = 32 * (ULB_EPI_WARPS + 1 + ULB_CTRL);
     B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, pl.smem));
     B200_REQUIRE((long long)per_sm * sm_count() >= pl.ctas, "bilstm(umma bwd): %d CTAs cannot be co-resident (%d/SM x %d SMs)",
                  pl.ctas, per_sm, sm_count());

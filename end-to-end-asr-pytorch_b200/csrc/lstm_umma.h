@@ -1,4 +1,4 @@
-// Internal interface of the tcgen05 BiLSTM step kernels (csrc/lstm_umma.cu), used by the C-ABI entry points in lstm.cu.
+// Internal interface of the wgmma BiLSTM step kernels (csrc/lstm_umma.cu), used by the C-ABI entry points in lstm.cu.
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>

@@ -8,7 +8,7 @@
 
 namespace b200asr {
 
-constexpr int NORM_BLOCKS = 592;  // 4 per SM on a 148-SM part
+constexpr int NORM_BLOCKS = 528;  // 4 per SM on a 132-SM part
 constexpr int NORM_THREADS = 256;
 
 __global__ void __launch_bounds__(NORM_THREADS) sumsq_partial_kernel(const float* __restrict__ g, long long n,

@@ -27,11 +27,11 @@ class DataParallel:
             os.environ.setdefault("MASTER_PORT", "29500")
             if backend == "nccl":
                 torch.cuda.set_device(self.local_rank)
-                # The LSTM step kernels are cooperative: 128 CTAs, one per SM, all co-resident - 20 of the 148 SMs stay
+                # The LSTM step kernels are cooperative: 128 CTAs, one per SM, all co-resident - 4 of the 132 SMs stay
                 # free.  An all-reduce with more CTAs than that cannot run NEXT to them, so the exchange of a layer's
-                # gradients serialises with the next layer's backward instead of hiding behind it (measured at 2 GPUs,
-                # cfg B: 67.5 ms/step with NCCL's default, 66.8 with 16, 67.1 with 8).
-                os.environ.setdefault("NCCL_MAX_CTAS", "16")
+                # gradients serialises with the next layer's backward instead of hiding behind it.  4 follows from the SM
+                # count alone: its cost in all-reduce bandwidth has not been measured.
+                os.environ.setdefault("NCCL_MAX_CTAS", "4")
             dist.init_process_group(backend=backend, rank=self.rank, world_size=self.world)
             self.backend = backend
 

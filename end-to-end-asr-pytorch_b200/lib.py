@@ -72,13 +72,7 @@ SIGNATURES = {
                                   c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_tf32_residual": (c_int, [_P, _P, c_longlong, _P]),
     "b200asr_gemm3x_tn_pre": (c_int, [_P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
-    "b200asr_gemm3x_nn_pre": (c_int, [_P, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t,
-                                      _P]),
     "b200asr_gemm3x_tn_pre2": (c_int, [_P, _P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
-    "b200asr_gemm3x_nn_pre2": (c_int, [_P, _P, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t,
-                                       _P]),
-    "b200asr_gemm3x_nt_pre": (c_int, [_P, _P, c_longlong, c_longlong, c_int, _P, _P, c_longlong, c_longlong, c_int, _P, c_int,
-                                      c_int, c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_split_tf32": (c_int, [_P, _P, _P, c_longlong, _P]),
     "b200asr_grad_norm_scratch_bytes": (c_size_t, []),
     "b200asr_grad_norm": (c_int, [_P, c_longlong, _P, _P, _P]),

@@ -81,7 +81,7 @@ class RNNLayer(nn.Module):
     """(Bi)LSTM + optional LayerNorm / dropout / time down-sampling / tanh projection (src/module.py:93-158).
 
     `self.layer` is a torch.nn.LSTM used purely as the parameter container (identical state_dict keys); the
-    recurrence itself runs in the persistent sm_100a kernels."""
+    recurrence itself runs in the persistent sm_90a kernels."""
 
     def __init__(self, input_dim, module, dim, bidirection, dropout, layer_norm, sample_rate, sample_style, proj):
         super().__init__()
@@ -98,7 +98,7 @@ class RNNLayer(nn.Module):
         self.module = module.upper()
         if self.module not in ("LSTM", "GRU"):
             raise NotImplementedError("RNN module %s (the reference accepts LSTM and GRU, src/module.py:112-113)" % module)
-        # LSTM: parameter container only, the recurrence runs in the persistent sm_100a kernels.  GRU (SURVEY.md 8(f)
+        # LSTM: parameter container only, the recurrence runs in the persistent sm_90a kernels.  GRU (SURVEY.md 8(f)
         # rank 4, no BASELINE config uses it): the library cuDNN layer, same state_dict keys as the reference.
         self.layer = getattr(nn, self.module)(input_dim, dim, bidirectional=bidirection, num_layers=1, batch_first=True)
         if self.layer_norm:

@@ -39,32 +39,22 @@ def gate_perm(H, device):
 # ----------------------------------------------------------------------------------------------------------
 # Dense contractions of the step (K6 / K9 / K11 and their autograd backward).  fp32 parity (1e-4 on logits after 4
 # recurrent layers) rules out single-pass TF32/BF16, so every product is error-compensated "3xTF32" (fp32 class).
-# GEMM_MODE "umma" (default): this library's own tcgen05 kernel (csrc/gemm.cu) in its three operand forms -
+# GEMM_MODE "umma" (default): this library's own wgmma kernel (csrc/gemm.cu) in its three operand forms -
 #   gemm_tn  x . W^T (+ bias)   forward;   gemm_nn  dY . W   input gradient (W in place);   gemm_nt  dY^T . X   weight
 #   gradient (contraction over the B*T rows, h_prev read shifted from the layer output, gate permutation in the epilogue).
-#   Raw fp32 tiles are the TF32 hi operands, residual tiles are made on the fly in shared memory, and the TMEM
-#   accumulation chain is cut every 128 k and summed in fp32 registers (the tensor core's own adds truncate).
+#   Raw fp32 tiles are the TF32 hi operands, residual tiles are made on the fly in shared memory, and the MMA
+#   accumulation chain is cut every 128 k and summed in a second fp32 register tile.
+#   A K-major operand (a and w of gemm_tn) may bring its residual pre-computed (tf32_residual: the weights, once per
+#   step); MN-major operands (w of gemm_nn, both operands of gemm_nt) pass through the kernel's transposing pass, which
+#   makes their residual anyway, so those forms take none.
 # GEMM_MODE "tf32x3": the same arithmetic as three cuBLAS TF32 GEMMs on operands split by b200asr_split_tf32 (kept as a
 #   cross-check and for shapes whose row pitch is not a multiple of 4 floats); "fp32": cuBLAS SGEMM on the CUDA cores.
 GEMM_MODE = os.environ.get("B200ASR_GEMM", "umma")
 
 
-# Pre-split activations too (B200ASR_GEMM_PRESPLIT):
-#   "x" (default)  only the wide operand of the weight-gradient products (the layer input x for dW_ih, the layer output
-#                  for dW_hh: small next to dG): nt 188 -> 204 TFLOP/s, cfg B weight gradients 13.5 -> 12.8 ms for 0.5 ms of
-#                  residual passes
-#   "1"            every activation / gradient operand (no in-kernel split pass at all): measured SLOWER (cfg B 66.1 ->
-#                  68.4 ms/step; tn 248 -> 232, nn 233 -> 208 TFLOP/s) - the extra residual tiles arrive through the same
-#                  L2 -> SM path that already runs at ~2/3 of its measured rate
-#   "0"            weights only
-_PRESPLIT = os.environ.get("B200ASR_GEMM_PRESPLIT", "x")
-PRESPLIT_ACTIVATIONS = _PRESPLIT == "1"
-PRESPLIT_NT_B = _PRESPLIT == "x"
-
-
 def tf32_residual(w):
     """w - trunc_tf32(w): the part of a weight matrix the tensor core does not see in the raw fp32 bit pattern.  Computed
-    once per step and weight (instead of once per tile by every CTA) for the `_pre` GEMM forms."""
+    once per step and weight (instead of once per tile by every CTA) for the pre-split forms of gemm_tn."""
     lib = L.load()
     w = _f32c(w)
     lo = torch.empty_like(w)
@@ -128,7 +118,7 @@ def gemm_tn_ld(a_base, lda, M, K, w, bias=None):
     return out
 
 
-def gemm_nn(a, w, out=None, accumulate=False, w_lo=None, a_lo=None):
+def gemm_nn(a, w, out=None, accumulate=False):
     """out[M,N] (= or +=) a[M,K] @ w[K,N]: the input gradient dY . W with W read in place (MN-major operand)."""
     lib = L.load()
     a, w = _f32c(a), _f32c(w)
@@ -139,19 +129,7 @@ def gemm_nn(a, w, out=None, accumulate=False, w_lo=None, a_lo=None):
         accumulate = False
     assert out.stride(1) == 1 and out.shape == (M, N)
     with L.timed("gemm3x_nn", 4 * (M * K + N * K + M * N * (2 if accumulate else 1))):
-        if w_lo is not None and a_lo is not None:
-            ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
-            ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
-            L.check(lib.b200asr_gemm3x_nn_pre2(L.ptr(a), L.ptr(a_lo), K, L.ptr(w), L.ptr(w_lo), N, None, L.ptr(out), M, N, K,
-                                               out.stride(0), int(bool(accumulate)), L.ptr(ws), ws_bytes, L.stream()),
-                    "gemm3x_nn_pre2")
-        elif w_lo is not None:
-            ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
-            ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
-            L.check(lib.b200asr_gemm3x_nn_pre(L.ptr(a), K, L.ptr(w), L.ptr(w_lo), N, None, L.ptr(out), M, N, K,
-                                              out.stride(0), int(bool(accumulate)), L.ptr(ws), ws_bytes, L.stream()),
-                    "gemm3x_nn_pre")
-        elif M <= 256:
+        if M <= 256:
             ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
             ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
             L.check(lib.b200asr_gemm3x_nn_ws(L.ptr(a), K, L.ptr(w), N, None, L.ptr(out), M, N, K, out.stride(0),
@@ -162,11 +140,9 @@ def gemm_nn(a, w, out=None, accumulate=False, w_lo=None, a_lo=None):
     return out
 
 
-def gemm_nt(a, b, M, N, T, batches=1, lda=None, a_bstride=0, ldb=None, b_bstride=0, b_shift=0, permute_rows=False,
-            a_lo=None, b_lo=None):
+def gemm_nt(a, b, M, N, T, batches=1, lda=None, a_bstride=0, ldb=None, b_bstride=0, b_shift=0, permute_rows=False):
     """out[M,N] = sum over (batch, t) of a[batch, t, :M]^T b[batch, t + b_shift, :N]: the weight gradient dY^T . X.
-    `a` / `b` are tensors whose data pointer is element (0, 0, 0); pitches are in floats (default: dense [T, M] / [T, N]).
-    b_lo (+ optionally a_lo): tf32_residual of the operands, same layout - their tiles are not split in the kernel."""
+    `a` / `b` are tensors whose data pointer is element (0, 0, 0); pitches are in floats (default: dense [T, M] / [T, N])."""
     lib = L.load()
     lda = M if lda is None else lda
     ldb = N if ldb is None else ldb
@@ -174,14 +150,9 @@ def gemm_nt(a, b, M, N, T, batches=1, lda=None, a_bstride=0, ldb=None, b_bstride
     ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
     ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
     with L.timed("gemm3x_nt", 4 * (batches * T * (M + N) + M * N)):
-        if b_lo is not None:
-            L.check(lib.b200asr_gemm3x_nt_pre(L.ptr(a), L.ptr(a_lo), lda, a_bstride, 0, L.ptr(b), L.ptr(b_lo), ldb, b_bstride,
-                                              b_shift, L.ptr(out), M, N, T, batches, N, 0, int(bool(permute_rows)),
-                                              L.ptr(ws), ws_bytes, L.stream()), "gemm3x_nt_pre")
-        else:
-            L.check(lib.b200asr_gemm3x_nt(L.ptr(a), lda, a_bstride, 0, L.ptr(b), ldb, b_bstride, b_shift, L.ptr(out), M, N,
-                                          T, batches, N, 0, int(bool(permute_rows)), L.ptr(ws), ws_bytes, L.stream()),
-                    "gemm3x_nt")
+        L.check(lib.b200asr_gemm3x_nt(L.ptr(a), lda, a_bstride, 0, L.ptr(b), ldb, b_bstride, b_shift, L.ptr(out), M, N,
+                                      T, batches, N, 0, int(bool(permute_rows)), L.ptr(ws), ws_bytes, L.stream()),
+                "gemm3x_nt")
     return out
 
 
@@ -339,18 +310,13 @@ class BiLSTMFn(Function):
         umma = _use_umma(I)
         xs = None if umma else Op(x.view(B * T, I))
         gates = torch.empty((ndir, B, T, H, 4), device=dev, dtype=torch.float32)
-        w_ih_p, w_ih_lo = [], []
-        # the layer input enters the forward projection of both directions and both dW_ih products: split it once
-        x_lo = tf32_residual(x) if (umma and PRESPLIT_ACTIVATIONS) else None
+        w_ih_p = []
         for d in range(ndir):
             w_ih, w_hh, b_ih, b_hh = params[4 * d:4 * d + 4]
             wp = w_ih.detach().index_select(0, perm)
             bp = (b_ih.detach() + b_hh.detach()).index_select(0, perm)
             if umma:
-                wlo = tf32_residual(wp)            # once per step: shared by the forward product and the input gradient
-                gemm_tn(x.view(B * T, I), wp, bias=bp, out=gates[d].view(B * T, 4 * H), w_lo=wlo,
-                        a_lo=x_lo.view(B * T, I) if x_lo is not None else None)
-                w_ih_lo.append(wlo)
+                gemm_tn(x.view(B * T, I), wp, bias=bp, out=gates[d].view(B * T, 4 * H), w_lo=tf32_residual(wp))
             else:
                 mm(xs, Op(wp).t(), out=gates[d].view(B * T, 4 * H), bias=bp)
             w_ih_p.append(wp)
@@ -369,8 +335,7 @@ class BiLSTMFn(Function):
         ctx.ndir = ndir
         ctx.dims = (B, T, I, H)
         ctx.consumed = False
-        ctx.has_x_lo = x_lo is not None
-        ctx.save_for_backward(x, gates, cst, out, w_hh, *w_ih_p, *w_ih_lo, *([x_lo] if x_lo is not None else []))
+        ctx.save_for_backward(x, gates, cst, out, w_hh, *w_ih_p)
         return out
 
     @staticmethod
@@ -384,9 +349,6 @@ class BiLSTMFn(Function):
         B, T, I, H = ctx.dims
         x, gates, cst, out, w_hh = ctx.saved_tensors[:5]
         w_ih_p = ctx.saved_tensors[5:5 + ndir]
-        rest = ctx.saved_tensors[5 + ndir:]
-        x_lo = rest[-1] if ctx.has_x_lo else None
-        w_ih_lo = rest[:-1] if ctx.has_x_lo else rest
         dev = x.device
         dout = _f32c(dout)
         ws_bytes = lib.b200asr_bilstm_workspace_bytes(B, T, H, ndir)
@@ -402,26 +364,14 @@ class BiLSTMFn(Function):
             # own tensor-core kernels throughout: dX = dG . W (W in place), dW_ih = dG^T . X, dW_hh = dG^T . h_prev with
             # h_prev read from the layer output shifted by one step (never materialised); rows written through the gate
             # permutation by the epilogue.
-            # Residuals made once per step (B200ASR_GEMM_PRESPLIT): "x" = the wide operand of the two weight-gradient
-            # products (layer input for dW_ih, layer output for dW_hh); "1" = the gate gradient as well (it enters
-            # dX, dW_ih and dW_hh), so that none of these kernels splits a tile - measured slower, see the switch above
-            pre = x_lo is not None and len(w_ih_lo) == ndir
-            g_lo = tf32_residual(gates) if pre else None
-            pre_b = pre or PRESPLIT_NT_B
-            if PRESPLIT_NT_B:
-                x_lo = tf32_residual(x)
-            out_lo = tf32_residual(out) if pre_b else None
             for d in range(ndir):
                 g2 = gates[d].view(B * T, 4 * H)
-                gl2 = g_lo[d].view(B * T, 4 * H) if pre else None
                 if need_dx:
-                    gemm_nn(g2, w_ih_p[d], out=dx2, accumulate=(d > 0), w_lo=w_ih_lo[d] if len(w_ih_lo) == ndir else None,
-                            a_lo=gl2)
-                dw_ih = gemm_nt(g2, x, 4 * H, I, B * T, permute_rows=True, a_lo=gl2, b_lo=x_lo)
+                    gemm_nn(g2, w_ih_p[d], out=dx2, accumulate=(d > 0))
+                dw_ih = gemm_nt(g2, x, 4 * H, I, B * T, permute_rows=True)
                 hd = out[:, :, d * H:(d + 1) * H]
                 dw_hh = gemm_nt(g2, hd, 4 * H, H, T, batches=B, a_bstride=T * 4 * H, ldb=ndir * H,
-                                b_bstride=T * ndir * H, b_shift=(-1 if d == 0 else 1), permute_rows=True,
-                                a_lo=gl2, b_lo=out_lo[:, :, d * H:(d + 1) * H] if pre_b else None)
+                                b_bstride=T * ndir * H, b_shift=(-1 if d == 0 else 1), permute_rows=True)
                 db = torch.empty((4 * H,), device=dev, dtype=torch.float32)
                 db.index_copy_(0, perm, g2.sum(0))
                 grads += [dw_ih, dw_hh, db, db.clone()]
@@ -748,18 +698,18 @@ class DecStepFn(Function):
         ctx.set_materialize_grads(False)
         xcat = torch.cat([x, h], 1).contiguous()
         pre = gemm_tn(xcat, wcat, bias=bias, w_lo=wlo)
-        ctx.save_for_backward(xcat, wcat, wlo)
+        ctx.save_for_backward(xcat, wcat)
         ctx.mem = mem
         ctx.I = x.shape[1]
         return pre
 
     @staticmethod
     def backward(ctx, dpre):
-        xcat, wcat, wlo = ctx.saved_tensors
+        xcat, wcat = ctx.saved_tensors
         if dpre is None:
             return None, None, None, None, None, None, None
         dpre = _f32c(dpre)
-        dx = gemm_nn(dpre, wcat, w_lo=wlo)
+        dx = gemm_nn(dpre, wcat)
         ctx.mem.dpre.append(dpre)
         ctx.mem.x.append(xcat)
         return None, torch.zeros(1, device=dpre.device), dx[:, :ctx.I], dx[:, ctx.I:], None, None, None
@@ -1021,14 +971,13 @@ class Linear3xFn(Function):
         Op, mm = _gemm_ops()
         shp = x.shape
         x2 = _f32c(x).reshape(-1, shp[-1])
-        wlo = None
         if _use_umma(x2.shape[1]):
-            wlo = tf32_residual(weight.detach())
-            y = gemm_tn(x2, weight.detach(), bias=bias.detach() if bias is not None else None, w_lo=wlo)
+            y = gemm_tn(x2, weight.detach(), bias=bias.detach() if bias is not None else None,
+                        w_lo=tf32_residual(weight.detach()))
         else:
             y = mm(Op(x2), Op(weight.detach()).t(), bias=bias.detach() if bias is not None else None,
                    out=torch.empty((x2.shape[0], weight.shape[0]), device=x.device, dtype=torch.float32))
-        ctx.save_for_backward(x2, weight, *([wlo] if wlo is not None else []))
+        ctx.save_for_backward(x2, weight)
         ctx.shp = shp
         ctx.has_bias = bias is not None
         return y.view(*shp[:-1], weight.shape[0])
@@ -1036,14 +985,13 @@ class Linear3xFn(Function):
     @staticmethod
     def backward(ctx, gy):
         Op, mm = _gemm_ops()
-        x2, weight = ctx.saved_tensors[:2]
-        wlo = ctx.saved_tensors[2] if len(ctx.saved_tensors) > 2 else None
+        x2, weight = ctx.saved_tensors
         gy2 = _f32c(gy).reshape(-1, weight.shape[0])
         dx = None
         umma = _use_umma(weight.shape[0]) and _use_umma(weight.shape[1])
         if ctx.needs_input_grad[0]:
             if umma:
-                dx = gemm_nn(gy2, weight.detach(), w_lo=wlo).view(ctx.shp)
+                dx = gemm_nn(gy2, weight.detach()).view(ctx.shp)
             else:
                 dx = mm(Op(gy2), Op(weight.detach())).view(ctx.shp)
         dw = None

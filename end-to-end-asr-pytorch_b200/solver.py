@@ -32,7 +32,7 @@ class BaseSolver:
             self.device = torch.device("cuda", torch.cuda.current_device())
         else:
             # the reference's --cpu path is the BASELINE (oracle/ref_port.py); this package has no CPU kernels
-            raise RuntimeError("the B200 solver needs a CUDA device; run the reference itself for --cpu")
+            raise RuntimeError("the GPU solver needs a CUDA device; run the reference itself for --cpu")
         self.amp = getattr(paras, "amp", False)
         if self.amp:
             raise NotImplementedError("--amp (apex) is not part of the fp32-parity hot path")

@@ -3,7 +3,7 @@
 `ASR.forward` in argmax-feedback mode over the dev and test sets and writes `<outdir>/<name>_{dev,test}_output.csv`
 (`idx<TAB>hyp<TAB>truth`).
 
-B200-native differences: raw audio goes to the GPU and the fused front end runs there (fetch_data); the arg-max token
+GPU-native differences: raw audio goes to the GPU and the fused front end runs there (fetch_data); the arg-max token
 ids of a whole batch are produced on the device (for CTC-only models by the log-softmax kernel itself,
 `ASR.last_ctc_argmax`) and leave it with ONE copy per batch instead of one `.tolist()` sync per utterance
 (bin/test_asr.py:113-118).  Beam search (`beam_size > 1`: src/decode.py, src/ctc.py) is CPU/numpy, batch 1, in the
@@ -44,7 +44,7 @@ class Solver(BaseSolver):
         self.greedy = self.config["decode"]["beam_size"] == 1
         if not self.greedy:
             raise NotImplementedError("beam_size > 1: beam / CTC-prefix search is the reference's CPU path "
-                                      "(src/decode.py, src/ctc.py); only greedy decoding runs on the B200 path")
+                                      "(src/decode.py, src/ctc.py); only greedy decoding runs on the GPU path")
         self.step = 0
 
     def fetch_data(self, data):

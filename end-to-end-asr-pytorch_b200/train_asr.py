@@ -1,7 +1,7 @@
 """Training Solver with the reference's interface (/root/reference/bin/train_asr.py:10-217):
 Solver(config, paras, mode).load_data() / .set_model() / .exec(), same loss assembly, validation and checkpoints.
-Differences that make it B200-native: waveforms go to the GPU and the fused front end runs there (fetch_data);
-CTC / CE / attention / LSTM are the sm_100a kernels; one process per GPU with a single NCCL grad all-reduce."""
+Differences that make it GPU-native: waveforms go to the GPU and the fused front end runs there (fetch_data);
+CTC / CE / attention / LSTM are the sm_90a kernels; one process per GPU with a single NCCL grad all-reduce."""
 import os
 
 import torch

@@ -1,8 +1,8 @@
-/* libb200asr.so - C ABI of the B200-native ASR train-step kernels (sm_100a).
+/* libb200asr.so - C ABI of the ASR train-step kernels (H100, sm_90a).
  *
  * The reference (Alexander-H-Liu/End-to-end-ASR-Pytorch) is 100% Python and has no FFI of its own: every
  * "kernel" is a stock torch / torchaudio call.  Each entry point below therefore cites the reference CALL SITE
- * (file:line under /root/reference, or kaldi.py = torchaudio/compliance/kaldi.py) whose arithmetic it replaces.
+ * (file:line of the reference checkout, or kaldi.py = torchaudio/compliance/kaldi.py) whose arithmetic it replaces.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless stated otherwise; tensors are contiguous row-major fp32,
@@ -139,8 +139,8 @@ B200ASR_API int b200asr_bilstm_plan(int B, int H, int ndir, int* unit_block, int
 /* 1 when the step GEMMs of this shape run on the tensor cores (3xTF32 mma), 0 for the packed-fp32-FMA kernels,
  * -1 when the shape has no decomposition */
 B200ASR_API int b200asr_bilstm_uses_tensor_cores(int B, int H, int ndir);
-/* 1 when the forward recurrence of this shape runs on the 5th-generation tensor cores (tcgen05.mma kind::f16 with
- * fp32 accumulators in TMEM and the fp16 hi/lo "2 x 2 block" split product, csrc/lstm_umma.cu), else 0 */
+/* 1 when the forward recurrence of this shape runs on warpgroup MMAs (wgmma f16 with
+ * fp32 accumulators in registers and the fp16 hi/lo "2 x 2 block" split product, csrc/lstm_umma.cu), else 0 */
 B200ASR_API int b200asr_bilstm_uses_tcgen05(int B, int H, int ndir);
 B200ASR_API int b200asr_bilstm_fwd(float* gates, const float* w_hh, float* cstate, float* out, int B, int T, int H, int ndir,
                        void* workspace, size_t workspace_bytes, b200asr_stream stream);
@@ -214,8 +214,8 @@ B200ASR_API int b200asr_adam_step(float* param, const float* grad, float* exp_av
  * proj_k / char_trans / pj Linear layers (src/asr.py:177,220,242-243; src/module.py:123,155) and their input gradients.
  *   C[M,N] (+)= A[M,K] . B[N,K]^T + bias[N]      A, B row-major with K contiguous (16-byte aligned, K % 4 == 0),
  *   C row-major with leading dimension ldc >= N; bias may be NULL; accumulate != 0 adds to the existing C.
- * tcgen05.mma kind::tf32 with error compensation: raw fp32 tiles are the TF32 hi operands (the tensor core truncates),
- * the residual tiles are produced on the fly in shared memory; three products per K block into one TMEM accumulator. */
+ * wgmma tf32 with error compensation: raw fp32 tiles are the TF32 hi operands (the tensor core truncates),
+ * the residual tiles are produced on the fly in shared memory; three products per K block into one register accumulator. */
 B200ASR_API int b200asr_gemm3x_supported(int M, int N, int K);
 B200ASR_API int b200asr_gemm3x_tn(const float* A, const float* B, const float* bias, float* C, int M, int N, int K, int ldc,
                       int accumulate, b200asr_stream stream);
@@ -251,33 +251,19 @@ B200ASR_API int b200asr_gemm3x_nt(const float* A, long long lda, long long a_bst
                       int ldc, int accumulate, int permute_rows, void* workspace, size_t workspace_bytes,
                       b200asr_stream stream);
 
-/* the tn / nn forms with a PRE-SPLIT B operand: B_lo = B - trunc_tf32(B) (b200asr_tf32_residual; same shape and pitch
- * as B) is the weight matrix' residual, computed once per step instead of once per tile by every CTA: its tile arrives
- * by TMA like B's, the in-kernel splitter pass shrinks to the A tile and 8 of the 12 tensor-core products of a K block
- * no longer wait for it.  workspace may be NULL.                                                                    */
+/* the tn form with PRE-SPLIT operands: B_lo = B - trunc_tf32(B) (b200asr_tf32_residual; same shape and pitch as B) is
+ * the weight matrix' residual, computed once per step instead of once per tile by every CTA: its tile arrives by TMA
+ * like B's and the in-kernel split pass shrinks to the A tile.  _pre2 takes A_lo = A - trunc_tf32(A) (shape and pitch
+ * of A) as well: no in-kernel split pass at all.  Same residuals and the same 12 products per K block as the other
+ * entry points.  workspace may be NULL.  Only K-major operands can bring a residual: the MN-major operands of the nn
+ * and nt forms go through the kernel's transposing pass, which makes their residual in the same sweep.            */
 B200ASR_API int b200asr_tf32_residual(const float* x, float* lo, long long n, b200asr_stream stream);
 B200ASR_API int b200asr_gemm3x_tn_pre(const float* A, int lda, const float* B, const float* B_lo, const float* bias, float* C,
                           int M, int N, int K, int ldc, int accumulate, void* workspace, size_t workspace_bytes,
                           b200asr_stream stream);
-B200ASR_API int b200asr_gemm3x_nn_pre(const float* A, int lda, const float* B, const float* B_lo, int ldb, const float* bias,
-                          float* C, int M, int N, int K, int ldc, int accumulate, void* workspace,
-                          size_t workspace_bytes, b200asr_stream stream);
-/* all three forms with BOTH operands pre-split: A_lo = A - trunc_tf32(A) has the shape and pitches of A (an activation
- * or gradient matrix that enters several products of the step - the layer input x: forward projection and dW_ih; the
- * gate gradient dG: dX, dW_ih and dW_hh - so one elementwise pass replaces the per-tile split in each of them).  The
- * kernel then has no splitter pass at all: the 12 products of a K block are issued as soon as the four tiles have
- * landed.  Same residuals and the same 12 products per K block as the other entry points (the issue order of the
- * products differs, so results agree to fp32 rounding, not bit for bit).                                            */
 B200ASR_API int b200asr_gemm3x_tn_pre2(const float* A, const float* A_lo, int lda, const float* B, const float* B_lo,
                            const float* bias, float* C, int M, int N, int K, int ldc, int accumulate, void* workspace,
                            size_t workspace_bytes, b200asr_stream stream);
-B200ASR_API int b200asr_gemm3x_nn_pre2(const float* A, const float* A_lo, int lda, const float* B, const float* B_lo, int ldb,
-                           const float* bias, float* C, int M, int N, int K, int ldc, int accumulate, void* workspace,
-                           size_t workspace_bytes, b200asr_stream stream);
-B200ASR_API int b200asr_gemm3x_nt_pre(const float* A, const float* A_lo, long long lda, long long a_bstride, int a_shift,
-                          const float* B, const float* B_lo, long long ldb, long long b_bstride, int b_shift, float* C,
-                          int M, int N, int T, int batches, int ldc, int accumulate, int permute_rows, void* workspace,
-                          size_t workspace_bytes, b200asr_stream stream);
 
 /* ---- K6 helper: split fp32 into a TF32-representable high part and the fp32 residual ---------------------------
  * hi = x rounded to TF32, lo = x - hi; used to run the input-projection (src/module.py:131, inside nn.LSTM) and the

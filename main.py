@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 # coding: utf-8
-"""Same command line as the reference's main.py (/root/reference/main.py:13-47), driving the B200-native Solver.
+"""Same command line as the reference's main.py (reference main.py:13-47), driving the GPU-native Solver.
     python main.py --config config/b200/cfgB_ctc_char.yaml [--njobs 0] [--seed 0] [--load ckpt]
     torchrun --nproc-per-node 8 --master-addr 127.0.0.1 main.py --config ...      (data parallel, one process per GPU)
 --test runs greedy decoding (decode.beam_size 1); --cpu hands the whole command line to the reference checkout
-(B200ASR_REFERENCE, default /root/reference) - this package has no CPU path; --lm is outside this hot path."""
+(the directory named by B200ASR_REFERENCE) - this package has no CPU path; --lm is outside this hot path."""
 import argparse
 import importlib
 import os
@@ -14,7 +14,7 @@ import numpy as np
 import torch
 import yaml
 
-parser = argparse.ArgumentParser(description="Training E2E asr (B200-native hot path).")
+parser = argparse.ArgumentParser(description="Training E2E asr (GPU-native hot path).")
 parser.add_argument("--config", type=str, help="Path to experiment config.")
 parser.add_argument("--name", default=None, type=str, help="Name for logging.")
 parser.add_argument("--logdir", default="log/", type=str, help="Logging path.")
@@ -41,10 +41,10 @@ def main():
     setattr(paras, "verbose", not paras.no_msg)
     if paras.cpu:
         # SURVEY.md 8(b): `--cpu` keeps routing to the REFERENCE implementation (the baseline run, main.py:30,45 there).
-        # It is not part of this repository: point B200ASR_REFERENCE at a checkout (default /root/reference).
-        ref = os.environ.get("B200ASR_REFERENCE", "/root/reference")
+        # It is not part of this repository: point B200ASR_REFERENCE at a checkout.
+        ref = os.environ.get("B200ASR_REFERENCE", "")
         if not os.path.isfile(os.path.join(ref, "main.py")):
-            raise SystemExit("--cpu runs the reference's own CPU path, but no reference checkout was found at %s "
+            raise SystemExit("--cpu runs the reference's own CPU path, but no reference checkout was found at %r "
                              "(set B200ASR_REFERENCE); this package has no CPU fallback" % ref)
         import runpy
         sys.path.insert(0, ref)
@@ -52,7 +52,7 @@ def main():
         sys.argv[0] = os.path.join(ref, "main.py")
         return runpy.run_path(sys.argv[0], run_name="__main__")
     if paras.lm or paras.cudnn_ctc:
-        raise SystemExit("--lm / --cudnn-ctc select reference paths outside the B200 hot path")
+        raise SystemExit("--lm / --cudnn-ctc select reference paths outside the GPU hot path")
     config = yaml.load(open(paras.config, "r"), Loader=yaml.FullLoader)
     np.random.seed(paras.seed)
     torch.manual_seed(paras.seed)

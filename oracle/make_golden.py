@@ -11,7 +11,7 @@ import sys
 import numpy as np
 import torch
 
-from . import ref_shim
+from . import golden_io, ref_shim
 
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
 
@@ -144,7 +144,7 @@ def golden_model(kind, seed, B, T, D, V, Lmax):
             _, _, g_out, g_seq, _ = model(feat, feat_len, int(txt_len.max()) + 2)
         out["greedy_argmax"] = g_out.argmax(-1).numpy()
         out["greedy_output"] = g_out.numpy()
-    np.savez_compressed(os.path.join(OUT, "model_%s.npz" % kind), **out)
+    golden_io.save(os.path.join(OUT, "model_%s.npz" % kind), out)
     print("model_%s.npz" % kind, "loss", float(total), "grad_norm", float(gn))
 
 

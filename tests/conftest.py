@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (select with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -32,7 +32,8 @@ def pkg():
 
 
 def load_golden(name):
-    return dict(np.load(os.path.join(GOLDEN, name), allow_pickle=False))
+    from oracle import golden_io
+    return golden_io.load(os.path.join(GOLDEN, name))
 
 
 def rel_err(a, b, floor=1e-3):

@@ -1,5 +1,5 @@
 """Parity of every CUDA kernel (through the C ABI) against the CPU oracle / committed golden vectors.
-Run on the B200 box: python -m pytest tests -m gpu."""
+Run with: python -m pytest tests -m gpu."""
 import numpy as np
 import pytest
 import torch
@@ -276,7 +276,7 @@ def test_bilstm_fp32_fma_kernels_on_the_large_shapes(pkg, B, T, I, H, bidir):
 
 @pytest.mark.parametrize("B,T,I,H,bidir", [(32, 11, 24, 640, True), (64, 10, 120, 512, True), (40, 9, 16, 512, False)])
 def test_bilstm_mma_sync_generation_on_the_large_shapes(pkg, B, T, I, H, bidir):
-    """The warp-level mma.sync 3xTF32 forward kernels (round 1) remain the path for shapes the tcgen05 kernel does
+    """The warp-level mma.sync 3xTF32 forward kernels (round 1) remain the path for shapes the wgmma kernel does
     not take (H % 64 != 0 ...); keep them covered at the BASELINE shapes by forcing them (mode 3)."""
     lib = pkg.load_library()
     lib.b200asr_debug_set_lstm_mode(3)
@@ -289,7 +289,7 @@ def test_bilstm_mma_sync_generation_on_the_large_shapes(pkg, B, T, I, H, bidir):
 
 @pytest.mark.parametrize("B,T,I,H,bidir", [(64, 10, 120, 512, True), (40, 9, 16, 512, False), (64, 300, 64, 512, True)])
 def test_bilstm_backward_generation_toggle(pkg, B, T, I, H, bidir):
-    """Mode flag 512 selects the OTHER backward generation than the default one (tcgen05 <-> mma.sync): both stay
+    """Mode flag 512 selects the OTHER backward generation than the default one (wgmma <-> mma.sync): both stay
     parity-tested at the BASELINE shape whichever is the default."""
     lib = pkg.load_library()
     lib.b200asr_debug_set_lstm_mode(512)
@@ -302,7 +302,7 @@ def test_bilstm_backward_generation_toggle(pkg, B, T, I, H, bidir):
 @pytest.mark.parametrize("B,T,I,H,bidir", [(64, 10, 120, 512, True), (32, 11, 24, 640, True), (40, 9, 16, 512, False),
                                            (8, 13, 40, 320, True), (64, 300, 64, 512, True)])
 def test_bilstm_exchange_protocol_toggle(pkg, B, T, I, H, bidir):
-    """Mode flags 1024 (forward) / 2048 (backward) select the OTHER state-exchange protocol of the tcgen05 kernels than
+    """Mode flags 1024 (forward) / 2048 (backward) select the OTHER state-exchange protocol of the wgmma kernels than
     the default one (data-is-the-flag polling <-> fence + counter + bulk copy): both stay parity-tested."""
     lib = pkg.load_library()
     lib.b200asr_debug_set_lstm_mode(1024 + 2048)
@@ -624,7 +624,7 @@ def test_ctc_prefix_score_vs_reference_scorer(pkg):
 @pytest.mark.parametrize("M,N,K,acc", [(3000, 2048, 1024, False), (300, 31, 120, False), (129, 257, 64, True),
                                       (1000, 5000, 2048, False), (77, 300, 2048, True), (5, 8, 4, False)])
 def test_gemm3x_umma_is_fp32_class(pkg, M, N, K, acc):
-    """csrc/gemm.cu (tcgen05 kind::tf32, raw tiles as hi + on-the-fly residual tiles, TMEM accumulator) must be as
+    """csrc/gemm.cu (wgmma tf32, raw tiles as hi + on-the-fly residual tiles, register accumulator) must be as
     accurate as an fp32 SGEMM against an fp64 product - incl. M / N / K tails, bias, accumulate and ldc > N."""
     torch.manual_seed(M + N)
     a = torch.randn(M, K, device=DEV)
@@ -669,7 +669,7 @@ def test_tf32_residual_pass(pkg, n):
 
 @pytest.mark.parametrize("B,T,C,O", [(3, 41, 120, 640), (2, 10, 640, 640)])
 def test_conv1d_k4s2_through_the_gemm_kernel(pkg, B, T, C, O):
-    """CNNExtractor's Conv1d(k=4, s=2, p=1) as one tcgen05 GEMM over the in-place im2col view (overlapping rows,
+    """CNNExtractor's Conv1d(k=4, s=2, p=1) as one wgmma GEMM over the in-place im2col view (overlapping rows,
     lda = 2C < K = 4C) against the library convolution in fp64: output, input gradient, weight / bias gradients."""
     torch.manual_seed(C + T)
     conv = torch.nn.Conv1d(C, O, 4, stride=2, padding=1)
@@ -745,14 +745,6 @@ def test_gemm3x_nn_is_fp32_class(pkg, M, N, K, acc):
     e3 = scaled_err(out.cpu().numpy(), ref.cpu().numpy())
     e1 = scaled_err(sg.cpu().numpy(), ref.cpu().numpy())
     assert e3 < 3e-6 and e3 < 20 * max(e1, 1e-7), (e3, e1)
-    out.copy_(c0)
-    pkg.ops.gemm_nn(a, b, out=out, accumulate=acc, w_lo=pkg.ops.tf32_residual(b))          # pre-split form
-    e3 = scaled_err(out.cpu().numpy(), ref.cpu().numpy())
-    assert e3 < 3e-6 and e3 < 20 * max(e1, 1e-7), (e3, e1)
-    out.copy_(c0)
-    pkg.ops.gemm_nn(a, b, out=out, accumulate=acc, w_lo=pkg.ops.tf32_residual(b), a_lo=pkg.ops.tf32_residual(a))
-    e3 = scaled_err(out.cpu().numpy(), ref.cpu().numpy())
-    assert e3 < 3e-6 and e3 < 20 * max(e1, 1e-7), (e3, e1)
 
 
 @pytest.mark.parametrize("M,N,T,batches,shift,perm", [
@@ -792,14 +784,4 @@ def test_gemm3x_nt_is_fp32_class(pkg, M, N, T, batches, shift, perm):
     assert torch.equal(out, out2)                                               # deterministic (split-K in fixed order)
     e3 = scaled_err(out.cpu().numpy(), ref.cpu().numpy())
     e1 = scaled_err(sg.cpu().numpy(), ref.cpu().numpy())
-    assert e3 < 3e-6 and e3 < 20 * max(e1, 1e-7), (e3, e1)
-    # both operands pre-split (the residual of the padded buffer has the operand's pitch)
-    out3 = pkg.ops.gemm_nt(a, bfull, M, N, T, batches=batches, a_bstride=T * M, ldb=ldb, b_bstride=T * ldb,
-                           b_shift=shift, permute_rows=perm, a_lo=pkg.ops.tf32_residual(a),
-                           b_lo=pkg.ops.tf32_residual(bfull))
-    e3 = scaled_err(out3.cpu().numpy(), ref.cpu().numpy())
-    assert e3 < 3e-6 and e3 < 20 * max(e1, 1e-7), (e3, e1)
-    out4 = pkg.ops.gemm_nt(a, bfull, M, N, T, batches=batches, a_bstride=T * M, ldb=ldb, b_bstride=T * ldb,
-                           b_shift=shift, permute_rows=perm, b_lo=pkg.ops.tf32_residual(bfull))      # B only
-    e3 = scaled_err(out4.cpu().numpy(), ref.cpu().numpy())
     assert e3 < 3e-6 and e3 < 20 * max(e1, 1e-7), (e3, e1)

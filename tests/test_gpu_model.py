@@ -1,4 +1,4 @@
-"""Model-level parity on the GPU: the reference's state_dict loaded into the B200 model must reproduce the
+"""Model-level parity on the GPU: the reference's state_dict loaded into the GPU model must reproduce the
 reference's outputs, losses, gradients and greedy ids (golden vectors from oracle/make_golden.py)."""
 import numpy as np
 import pytest

@@ -1,5 +1,5 @@
 """N-GPU data parallelism of the product path == the 1-GPU step on the global batch (needs >= 2 GPUs: run with
-`gpurun --gpus 2 -- python -m pytest tests/test_gpu_zz_dp.py -m gpu`; skipped on a 1-GPU box)."""
+`python -m pytest tests/test_gpu_zz_dp.py -m gpu` on a machine with two GPUs; skipped with one)."""
 import os
 import socket
 import subprocess

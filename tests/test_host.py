@@ -54,7 +54,7 @@ def test_lstm_plan_fills_the_sms(pkg, B, H, ndir, mode, exp):
     try:
         assert lib.b200asr_bilstm_plan(B, H, ndir, byref(ub), byref(bc), byref(n)) == 0
         assert (ub.value, bc.value, n.value) == exp
-        assert n.value <= 148 and H % ub.value == 0
+        assert n.value <= 132 and H % ub.value == 0
         assert lib.b200asr_bilstm_workspace_bytes(B, 100, H, ndir) > 0
     finally:
         lib.b200asr_debug_set_lstm_mode(0)
@@ -112,7 +112,7 @@ def test_init_adadelta_matches_reference_quirks(pkg):
 
 
 def test_lstm_planner_sweep_is_consistent(pkg):
-    """Every (B, H, ndir) either has a plan that fits the machine (<= 148 co-resident CTAs, unit block divides H,
+    """Every (B, H, ndir) either has a plan that fits the machine (<= 132 co-resident CTAs, unit block divides H,
     a workspace size, tensor-core flag in {0,1}) or is refused with rc < 0 and a message - never a crash or a zero."""
     from ctypes import c_int, byref
     lib = pkg.load_library()
@@ -128,7 +128,7 @@ def test_lstm_planner_sweep_is_consistent(pkg):
                     refused += 1
                     assert rc < 0 and tc == -1 and ws == 0 and "no feasible decomposition" in pkg.lib.last_error()
                     continue
-                assert 1 <= n.value <= 148 and H % ub.value == 0 and 4 <= bc.value <= 64 and ws > 0
+                assert 1 <= n.value <= 132 and H % ub.value == 0 and 4 <= bc.value <= 64 and ws > 0
                 assert tc in (0, 1)
                 if tc:
                     assert bc.value == 32 and ub.value % 2 == 0 and ub.value <= 16 and H % 32 == 0

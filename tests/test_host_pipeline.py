@@ -12,7 +12,7 @@ from conftest import GOLDEN, ROOT, load_golden
 
 
 def test_character_encoder_known_answers(pkg):
-    """/root/reference/tests/test_text.py:26-27: 'SPEECH LAB!' -> [22,19,8,8,6,11,3,15,4,5,2,1], vocab 31."""
+    """reference tests/test_text.py:26-27: 'SPEECH LAB!' -> [22,19,8,8,6,11,3,15,4,5,2,1], vocab 31."""
     enc = pkg.text.load_text_encoder("character", os.path.join(GOLDEN, "character.vocab"))
     assert enc.vocab_size == 31 and enc.token_type == "character"
     ids = enc.encode("SPEECH LAB!")
@@ -80,7 +80,7 @@ def _dp_worker(rank, world, port, out):
     from oracle import ref_port
     from oracle.make_golden import tiny_model_cfg
     dp = pkg.dist.DataParallel(backend="gloo")
-    g = dict(np.load(os.path.join(GOLDEN, "model_hybrid.npz")))
+    g = load_golden("model_hybrid.npz")
     cfg = tiny_model_cfg("hybrid")
     P = {k[3:]: torch.from_numpy(v).clone().requires_grad_(True) for k, v in g.items() if k.startswith("sd.")}
     feat, flen, txt = torch.from_numpy(g["feat"]), torch.from_numpy(g["feat_len"]), torch.from_numpy(g["txt"])

@@ -1,5 +1,5 @@
 """Full-size BiLSTM layer (B=64, T=1198, I=120, H=512): gradients of the three backward variants against each other
-(default = tcgen05 + polling exchange, 2048 = tcgen05 + flag exchange, 512 = mma.sync generation) and, for scale,
+(default = wgmma + polling exchange, 2048 = wgmma + flag exchange, 512 = mma.sync generation) and, for scale,
 against an fp64 CPU LSTM on the first rows.  Prints max-abs differences relative to each tensor's max."""
 import importlib, os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -11,7 +11,7 @@ x0 = torch.randn(B, T, I)
 gy = torch.randn(B, T, 2 * H) * 0.01
 lib = pkg.lib.load()
 res = {}
-for mode, name in ((0, "tcgen05+poll"), (2048, "tcgen05+flag"), (512, "mma.sync"), (0, "tcgen05+poll again")):
+for mode, name in ((0, "wgmma+poll"), (2048, "wgmma+flag"), (512, "mma.sync"), (0, "wgmma+poll again")):
     lib.b200asr_debug_set_lstm_mode(mode)
     params = [p.detach().cuda().requires_grad_(True) for p in ref.parameters()]
     x = x0.cuda().requires_grad_(True)
@@ -34,7 +34,7 @@ x32 = x0.clone().requires_grad_(True)
 y32, _ = r32(x32)
 y32.backward(gy)
 res["aten-cpu-fp32"] = [x32.grad.double()] + [p.grad.double() for p in r32.parameters()]
-for a in ("tcgen05+poll", "tcgen05+flag", "mma.sync", "tcgen05+poll again", "aten-cpu-fp32"):
+for a in ("wgmma+poll", "wgmma+flag", "mma.sync", "wgmma+poll again", "aten-cpu-fp32"):
     print("== %s vs fp64" % a)
     for n, u, v in zip(names, res[a], res["fp64"]):
         print("   %-28s %.3e" % (n, float((u - v).abs().max() / v.abs().max())))

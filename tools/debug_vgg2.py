@@ -2,7 +2,8 @@
 import os, sys, numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-g = dict(np.load(os.path.join(ROOT, "tests", "golden", "model_vgg.npz")))
+from oracle import golden_io
+g = golden_io.load(os.path.join(ROOT, "tests", "golden", "model_vgg.npz"))
 def build():
     c0, c1 = 64, 128
     ext = torch.nn.Sequential(

@@ -1,10 +1,9 @@
-"""SASS mnemonic counts per kernel of the built library (static evidence that the tcgen05 / TMA paths are what ships).
-usage: python tools/sass_mnemonics.py > profiles/rNN_sass_mnemonics.txt   (needs cuobjdump + c++filt; no GPU)"""
+"""SASS mnemonic counts per kernel of the built library (static evidence that the wgmma / TMA paths are what ships).
+usage: python tools/sass_mnemonics.py   (needs cuobjdump + c++filt; no GPU)"""
 import os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 so = os.path.join(ROOT, "end-to-end-asr-pytorch_b200", "libb200asr.so")
-MN = ["UTCHMMA", "UTCQMMA", "UTCMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "UBLKCP", "SYNCS", "HMMA", "FFMA2", "LDGSTS",
-      "UTCATOMSWS", "UTMACCTL"]
+MN = ["HGMMA", "UTMALDG", "UBLKCP", "SYNCS", "HMMA", "LDGSTS", "UTMACCTL"]
 
 
 def mnemonic_counts(path=so):
@@ -32,8 +31,8 @@ def mnemonic_counts(path=so):
 
 
 if __name__ == "__main__":
-    print("SASS mnemonic counts per kernel of libb200asr.so (cuobjdump -sass, sm_100a): tcgen05.mma = UTC*MMA, tcgen05.ld = LDTM,")
-    print("cp.async.bulk.tensor = UTMALDG, cp.async.bulk = UBLKCP, cp.async = LDGSTS, mbarrier = SYNCS, tcgen05.commit = UTCBAR, mma.sync = HMMA")
+    print("SASS mnemonic counts per kernel of libb200asr.so (cuobjdump -sass, sm_90a): wgmma = HGMMA,")
+    print("cp.async.bulk.tensor = UTMALDG, cp.async.bulk = UBLKCP, cp.async = LDGSTS, mbarrier = SYNCS, mma.sync = HMMA")
     print("%-78s" % "kernel" + "".join("%9s" % k for k in MN))
     for nice, c in sorted(mnemonic_counts().items()):
         if any(c.values()):

@@ -1,4 +1,4 @@
-"""ms / effective TFLOP/s of the own tcgen05 3xTF32 GEMM forms (tn, nn, nt) at the cfg-B layer shapes, next to the cuBLAS
+"""ms / effective TFLOP/s of the own wgmma 3xTF32 GEMM forms (tn, nn, nt) at the cfg-B layer shapes, next to the cuBLAS
 3xTF32 composition (3 library GEMMs + split passes) and a single cuBLAS TF32 GEMM (not fp32-class; speed reference)."""
 import importlib, os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -44,20 +44,12 @@ for M, N, K in shapes:
     wlo = ops.tf32_residual(w)
     tp = timeit(lambda: ops.gemm_tn(x, w, w_lo=wlo))
     print("tn  pre-split W                              own %7.3f ms (%6.1f TF)" % (tp, fl / tp), flush=True)
-    tp = timeit(lambda: ops.gemm_nn(dy, w, w_lo=wlo))
-    print("nn  pre-split W                              own %7.3f ms (%6.1f TF)" % (tp, fl / tp), flush=True)
-    xlo, dylo = ops.tf32_residual(x), ops.tf32_residual(dy)
+    xlo = ops.tf32_residual(x)
     tp = timeit(lambda: ops.gemm_tn(x, w, w_lo=wlo, a_lo=xlo))
     print("tn  both operands pre-split                  own %7.3f ms (%6.1f TF)" % (tp, fl / tp), flush=True)
-    tp = timeit(lambda: ops.gemm_nn(dy, w, w_lo=wlo, a_lo=dylo))
-    print("nn  both operands pre-split                  own %7.3f ms (%6.1f TF)" % (tp, fl / tp), flush=True)
-    tp = timeit(lambda: ops.gemm_nt(dy, x, N, K, M, a_lo=dylo, b_lo=xlo))
-    print("nt  both operands pre-split                  own %7.3f ms (%6.1f TF)" % (tp, fl / tp), flush=True)
-    tp = timeit(lambda: ops.gemm_nt(dy, x, N, K, M, b_lo=xlo))
-    print("nt  B (= x) pre-split only                   own %7.3f ms (%6.1f TF)" % (tp, fl / tp), flush=True)
     tp = timeit(lambda: ops.tf32_residual(dy))
     print("    residual pass over dy [%d x %d]          %7.3f ms" % (M, N, tp), flush=True)
-    del xlo, dylo
+    del xlo
     t2 = timeit(lambda: lib3(x, w.t()))
     t3 = timeit(lambda: tf32(x, w.t()))
     print("tn  y=x.W^T   M=%6d N=%5d K=%5d  own %7.3f ms (%6.1f TF)  cublas3x %7.3f ms  cublas-tf32x1 %7.3f ms" % (M, N, K, t, fl / t, t2, t3), flush=True)

@@ -1,4 +1,4 @@
-"""Per-step time of the BiLSTM step-kernel families (tcgen05 / mma.sync 3xTF32 / packed fp32 FMA) at one shape.
+"""Per-step time of the BiLSTM step-kernel families (wgmma / mma.sync 3xTF32 / packed fp32 FMA) at one shape.
    env: B (64), H (512), T (300), I (1024).  Prints us/step for forward and backward and the max |difference| of the
    outputs / input gradients between the two families."""
 import importlib, os, sys, torch
@@ -13,11 +13,11 @@ x = torch.randn(B, T, I, device="cuda", requires_grad=True)
 gy = torch.randn(B, T, 2 * H, device="cuda")
 lib = L.load()
 res = {}
-MODES = ((3, "mma.sync"), (0, "tcgen05"), (512, "tcgen05+bwd-toggle"), (3072, "tcgen05+exchange-toggle"))
+MODES = ((3, "mma.sync"), (0, "wgmma"), (512, "wgmma+bwd-toggle"), (3072, "wgmma+exchange-toggle"))
 if os.environ.get("ONLY_MODES"):
     MODES = tuple(m for m in MODES if str(m[0]) in os.environ["ONLY_MODES"].split(","))
 if os.environ.get("EXTRA_MODE"):
-    MODES += ((int(os.environ["EXTRA_MODE"]), "tcgen05-mode%s" % os.environ["EXTRA_MODE"]),)
+    MODES += ((int(os.environ["EXTRA_MODE"]), "wgmma-mode%s" % os.environ["EXTRA_MODE"]),)
 REPS = int(os.environ.get("REPS", 3))
 stats = {name: [] for _, name in MODES}
 fwd_only = {name: [] for _, name in MODES}
