@@ -42,11 +42,12 @@ def gate_perm(H, device):
 # GEMM_MODE "umma" (default): this library's own wgmma kernel (csrc/gemm.cu) in its three operand forms -
 #   gemm_tn  x . W^T (+ bias)   forward;   gemm_nn  dY . W   input gradient (W in place);   gemm_nt  dY^T . X   weight
 #   gradient (contraction over the B*T rows, h_prev read shifted from the layer output, gate permutation in the epilogue).
-#   Raw fp32 tiles are the TF32 hi operands, residual tiles are made on the fly in shared memory, and the MMA
-#   accumulation chain is cut every 128 k and summed in a second fp32 register tile.
-#   A K-major operand (a and w of gemm_tn) may bring its residual pre-computed (tf32_residual: the weights, once per
-#   step); MN-major operands (w of gemm_nn, both operands of gemm_nt) pass through the kernel's transposing pass, which
-#   makes their residual anyway, so those forms take none.
+#   A is split into hi / lo in registers (wgmma with A from registers); B's raw fp32 tile is its TF32 hi operand and
+#   its residual is made on the fly in shared memory, and the MMA accumulation chain is cut every 128 k and summed in
+#   a second fp32 register tile.
+#   The K-major w of gemm_tn may bring its residual pre-computed (tf32_residual: the weights, once per
+#   step); an MN-major B (w of gemm_nn, b of gemm_nt) passes through the kernel's transposing pass, which makes its
+#   residual anyway, and gemm_nt's a is gathered into registers with transposed addressing, so those forms take none.
 # GEMM_MODE "tf32x3": the same arithmetic as three cuBLAS TF32 GEMMs on operands split by b200asr_split_tf32 (kept as a
 #   cross-check and for shapes whose row pitch is not a multiple of 4 floats); "fp32": cuBLAS SGEMM on the CUDA cores.
 GEMM_MODE = os.environ.get("B200ASR_GEMM", "umma")
@@ -65,8 +66,8 @@ def tf32_residual(w):
 
 def gemm_tn(a, w, bias=None, out=None, accumulate=False, w_lo=None, a_lo=None):
     """out[M,N] (= or +=) a[M,K] @ w[N,K]^T (+ bias[N]) on the tensor cores at fp32-class accuracy (csrc/gemm.cu).
-    w_lo = tf32_residual(w) selects the pre-split form; a_lo = tf32_residual(a) in addition the form without any
-    in-kernel split pass."""
+    w_lo = tf32_residual(w) selects the pre-split form.  a_lo = tf32_residual(a) selects the pre2 entry point, which
+    computes the same products: the kernel makes A's residual in registers either way."""
     lib = L.load()
     a, w = _f32c(a), _f32c(w)
     M, K = a.shape
@@ -361,13 +362,15 @@ class BiLSTMFn(Function):
         dx2 = torch.empty((B * T, I), device=dev, dtype=torch.float32) if need_dx else None
         grads = []
         if _use_umma(I) and H % 4 == 0:
-            # own tensor-core kernels throughout: dX = dG . W (W in place), dW_ih = dG^T . X, dW_hh = dG^T . h_prev with
-            # h_prev read from the layer output shifted by one step (never materialised); rows written through the gate
-            # permutation by the epilogue.
+            # own tensor-core kernels throughout: dX = dG . W as the tn form on W^T (one transposed copy and its residual
+            # per layer and direction, so the kernel neither transposes nor splits the weight in every CTA),
+            # dW_ih = dG^T . X, dW_hh = dG^T . h_prev with h_prev read from the layer output shifted by one step (never
+            # materialised); rows written through the gate permutation by the epilogue.
             for d in range(ndir):
                 g2 = gates[d].view(B * T, 4 * H)
                 if need_dx:
-                    gemm_nn(g2, w_ih_p[d], out=dx2, accumulate=(d > 0))
+                    wt = w_ih_p[d].t().contiguous()
+                    gemm_tn(g2, wt, out=dx2, accumulate=(d > 0), w_lo=tf32_residual(wt))
                 dw_ih = gemm_nt(g2, x, 4 * H, I, B * T, permute_rows=True)
                 hd = out[:, :, d * H:(d + 1) * H]
                 dw_hh = gemm_nt(g2, hd, 4 * H, H, T, batches=B, a_bstride=T * 4 * H, ldb=ndir * H,

@@ -214,8 +214,9 @@ B200ASR_API int b200asr_adam_step(float* param, const float* grad, float* exp_av
  * proj_k / char_trans / pj Linear layers (src/asr.py:177,220,242-243; src/module.py:123,155) and their input gradients.
  *   C[M,N] (+)= A[M,K] . B[N,K]^T + bias[N]      A, B row-major with K contiguous (16-byte aligned, K % 4 == 0),
  *   C row-major with leading dimension ldc >= N; bias may be NULL; accumulate != 0 adds to the existing C.
- * wgmma tf32 with error compensation: raw fp32 tiles are the TF32 hi operands (the tensor core truncates),
- * the residual tiles are produced on the fly in shared memory; three products per K block into one register accumulator. */
+ * wgmma tf32 with error compensation: A is split into hi / lo in registers, B's raw fp32 tile is its TF32 hi operand
+ * (the tensor core truncates) and its residual tile is produced on the fly in shared memory; three products per K
+ * block into one register accumulator. */
 B200ASR_API int b200asr_gemm3x_supported(int M, int N, int K);
 B200ASR_API int b200asr_gemm3x_tn(const float* A, const float* B, const float* bias, float* C, int M, int N, int K, int ldc,
                       int accumulate, b200asr_stream stream);
@@ -253,10 +254,11 @@ B200ASR_API int b200asr_gemm3x_nt(const float* A, long long lda, long long a_bst
 
 /* the tn form with PRE-SPLIT operands: B_lo = B - trunc_tf32(B) (b200asr_tf32_residual; same shape and pitch as B) is
  * the weight matrix' residual, computed once per step instead of once per tile by every CTA: its tile arrives by TMA
- * like B's and the in-kernel split pass shrinks to the A tile.  _pre2 takes A_lo = A - trunc_tf32(A) (shape and pitch
- * of A) as well: no in-kernel split pass at all.  Same residuals and the same 12 products per K block as the other
- * entry points.  workspace may be NULL.  Only K-major operands can bring a residual: the MN-major operands of the nn
- * and nt forms go through the kernel's transposing pass, which makes their residual in the same sweep.            */
+ * like B's and no shared-memory split pass runs.  _pre2 takes A_lo = A - trunc_tf32(A) (shape and pitch of A) as
+ * well; the kernel makes the same values in registers, so it computes exactly what _pre computes.  Same residuals and
+ * the same 12 products per K block as the other entry points.  workspace may be NULL.  Only a K-major B can bring a
+ * residual: the MN-major B of the nn and nt forms goes through the kernel's transposing pass, which makes its
+ * residual in the same sweep.                                                                                     */
 B200ASR_API int b200asr_tf32_residual(const float* x, float* lo, long long n, b200asr_stream stream);
 B200ASR_API int b200asr_gemm3x_tn_pre(const float* A, int lda, const float* B, const float* B_lo, const float* bias, float* C,
                           int M, int N, int K, int ldc, int accumulate, void* workspace, size_t workspace_bytes,

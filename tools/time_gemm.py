@@ -1,13 +1,18 @@
-"""ms / effective TFLOP/s of the own wgmma 3xTF32 GEMM forms (tn, nn, nt) at the cfg-B layer shapes, next to the cuBLAS
-3xTF32 composition (3 library GEMMs + split passes) and a single cuBLAS TF32 GEMM (not fp32-class; speed reference)."""
-import importlib, os, sys, torch
+"""ms and TFLOP/s of the own wgmma 3xTF32 GEMM at the calls one cfg-B train step makes per BiLSTM layer and direction
+(input projection, input gradient and the transposed weight copy it needs, dW_ih, shifted dW_hh), with the share of
+the fp32-class ceiling: 3xTF32 runs three TF32 passes, so the ceiling is a third of the data-sheet dense TF32 rate (495 / 3 = 165 TFLOP/s on an H100 SXM at
+700 W).  Prints the card name and power limit of the run.  QUICK=1 times layer 3 only."""
+import importlib, os, subprocess, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 pkg = importlib.import_module("end-to-end-asr-pytorch_b200")
 ops = pkg.ops
 dev = "cuda"
+CEILING = 495.0 / 3        # TFLOP/s: H100 SXM data-sheet dense TF32 / 3 passes (a data-sheet figure, not measured)
+H, B = 512, 64             # cfg B: hidden size per direction, utterances per step
+LAYERS = [(76672, 120), (76672, 1024), (38336, 2048), (19136, 2048)]      # (B*T rows, input width) per layer
 
 
-def timeit(fn, reps=5):
+def timeit(fn, reps=10):
     for _ in range(2):
         fn()
     torch.cuda.synchronize()
@@ -20,42 +25,41 @@ def timeit(fn, reps=5):
     return e0.elapsed_time(e1) / reps
 
 
-def lib3(a, b_t):
-    return ops.mm3(ops.Split(a), ops.Split(b_t))
-
-
-def tf32(a, b):
-    torch.backends.cuda.matmul.allow_tf32 = True
-    try:
-        return a @ b
-    finally:
-        torch.backends.cuda.matmul.allow_tf32 = False
-
-
-shapes = [(76672, 2048, 120), (38336, 2048, 2048), (19168, 2048, 2048), (9584, 2048, 2048)]
-if os.environ.get("QUICK"):
-    shapes = shapes[1:2]
-for M, N, K in shapes:
-    x = torch.randn(M, K, device=dev)
-    w = torch.randn(N, K, device=dev) * 0.05
-    dy = torch.randn(M, N, device=dev)
-    fl = 2.0 * M * N * K / 1e9
-    t = timeit(lambda: ops.gemm_tn(x, w))
+q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
+                    str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+print("card: %s (name, power limit)" % (q or torch.cuda.get_device_name()))
+print("%-34s %6s %5s %5s %8s %8s %7s" % ("call", "M", "N", "K", "ms", "TFLOP/s", "ceiling"))
+layers = LAYERS[3:] if os.environ.get("QUICK") else LAYERS
+step_ms = step_tf = 0.0
+for li, (rows, I) in ((i, l) for i, l in enumerate(LAYERS) if l in layers):
+    T = rows // B
+    x = torch.randn(rows, I, device=dev)
+    w = torch.randn(4 * H, I, device=dev) * 0.05
+    g = torch.randn(rows, 4 * H, device=dev)
+    h = torch.randn(B, T, 2 * H, device=dev)
     wlo = ops.tf32_residual(w)
-    tp = timeit(lambda: ops.gemm_tn(x, w, w_lo=wlo))
-    print("tn  pre-split W                              own %7.3f ms (%6.1f TF)" % (tp, fl / tp), flush=True)
-    xlo = ops.tf32_residual(x)
-    tp = timeit(lambda: ops.gemm_tn(x, w, w_lo=wlo, a_lo=xlo))
-    print("tn  both operands pre-split                  own %7.3f ms (%6.1f TF)" % (tp, fl / tp), flush=True)
-    tp = timeit(lambda: ops.tf32_residual(dy))
-    print("    residual pass over dy [%d x %d]          %7.3f ms" % (M, N, tp), flush=True)
-    del xlo
-    t2 = timeit(lambda: lib3(x, w.t()))
-    t3 = timeit(lambda: tf32(x, w.t()))
-    print("tn  y=x.W^T   M=%6d N=%5d K=%5d  own %7.3f ms (%6.1f TF)  cublas3x %7.3f ms  cublas-tf32x1 %7.3f ms" % (M, N, K, t, fl / t, t2, t3), flush=True)
-    t = timeit(lambda: ops.gemm_nn(dy, w))
-    t2 = timeit(lambda: lib3(dy, w))
-    print("nn  dx=dy.W   M=%6d N=%5d K=%5d  own %7.3f ms (%6.1f TF)  cublas3x %7.3f ms" % (M, K, N, t, fl / t, t2), flush=True)
-    t = timeit(lambda: ops.gemm_nt(dy, x, N, K, M))
-    t2 = timeit(lambda: lib3(dy.t(), x))
-    print("nt  dW=dy^T.x M=%6d N=%5d K=%5d  own %7.3f ms (%6.1f TF)  cublas3x %7.3f ms" % (N, K, M, t, fl / t, t2), flush=True)
+    wt = w.t().contiguous()
+    wtlo = ops.tf32_residual(wt)
+    calls = [("L%d input projection tn (pre-split W)" % li, rows, 4 * H, I,
+              lambda: ops.gemm_tn(x, w, w_lo=wlo))]
+    if li > 0:                                   # the encoder input needs no gradient
+        calls += [("L%d W^T copy + its residual" % li, 0, 0, 0, lambda: ops.tf32_residual(w.t().contiguous())),
+                  ("L%d dX tn on W^T (pre-split)" % li, rows, I, 4 * H, lambda: ops.gemm_tn(g, wt, w_lo=wtlo)),
+                  ("L%d dX nn (W in place)" % li, rows, I, 4 * H, lambda: ops.gemm_nn(g, w))]
+    calls += [("L%d dW_ih nt" % li, 4 * H, I, rows, lambda: ops.gemm_nt(g, x, 4 * H, I, rows, permute_rows=True)),
+              ("L%d dW_hh nt (h_prev shifted)" % li, 4 * H, H, rows,
+               lambda: ops.gemm_nt(g, h, 4 * H, H, T, batches=B, a_bstride=T * 4 * H, ldb=2 * H, b_bstride=T * 2 * H,
+                                   b_shift=-1, permute_rows=True))]
+    for name, M, N, K, fn in calls:
+        ms = timeit(fn)
+        tf = 2.0 * M * N * K / ms / 1e9
+        if M == 0:                               # the input gradient's weight preparation (memory-bound, no FLOPs)
+            print("%-34s %26.3f" % (name, ms), flush=True)
+        else:
+            print("%-34s %6d %5d %5d %8.3f %8.1f %6.1f%%" % (name, M, N, K, ms, tf, 100 * tf / CEILING), flush=True)
+        if "nn" not in name:                     # the step runs the tn form of dX; nn is listed for comparison
+            step_ms += 2 * ms
+            step_tf += 2 * 2.0 * M * N * K / 1e12
+    del x, w, g, h, wlo, wt, wtlo
+print("sum over both directions: %.1f ms for %.2f TFLOP = %.1f TFLOP/s (%.1f%% of the %.0f TFLOP/s ceiling)"
+      % (step_ms, step_tf, step_tf / step_ms * 1e3, 100 * step_tf / step_ms * 1e3 / CEILING, CEILING))
