@@ -15,6 +15,7 @@
 // Restates /root/reference/src/module.py:234-258 (LocationAwareAttention.forward) + :189-195 (_attend), one head.
 #include "common.cuh"
 #include "../../include/b200asr.h"
+#include "../../include/b200asr_debug.h"
 #include <cooperative_groups.h>
 
 namespace cg = cooperative_groups;
@@ -497,6 +498,16 @@ extern "C" int b200asr_locattn_fwd(const float* q, const float* key, const float
     return launch_attn((const void*)locattn_fwd_kernel, p, threads, smem, (cudaStream_t)stream);
 }
 
+// MINB of the backward kernel: 2 when the CTAs outnumber the SMs and the smaller register budget fits the shape
+static int locattn_bwd_minb(int B, int T, int D, int E) {
+    const int cs = pick_cluster(T, E);
+    return ((long long)B * cs > sm_count() && D <= 384 && E / cs <= 512) ? 2 : 1;
+}
+
+extern "C" int b200asr_debug_locattn_bwd_minb(int B, int T, int D, int E) {
+    return (B > 0 && T > 0 && E > 0) ? locattn_bwd_minb(B, T, D, E) : 0;
+}
+
 static int locattn_bwd_impl(const float* q, const float* key, const float* value, const float* prev_att,
                             const long long* enc_len, const float* w_conv, const float* w_proj,
                             const float* w_energy, float temperature, const float* attn, const float* dctx,
@@ -522,7 +533,7 @@ static int locattn_bwd_impl(const float* q, const float* key, const float* value
     const size_t smem = sizeof(float) * ((size_t)T + 2 * R + (size_t)K * W + (size_t)D * K + 2 * D + 2 * (size_t)T +
                                          (size_t)p.CS * T + (size_t)K * ATT_TT + (size_t)ATT_TT * D +
                                          (size_t)K * (T + 2 * R));
-    const bool two_per_sm = (long long)B * p.CS > sm_count() && D <= 384 && E / p.CS <= 512;
+    const bool two_per_sm = locattn_bwd_minb(B, T, D, E) == 2;
     return launch_attn(two_per_sm ? (const void*)locattn_bwd_kernel<2> : (const void*)locattn_bwd_kernel<1>, p, threads,
                        smem, (cudaStream_t)stream);
 }

@@ -27,7 +27,7 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_kernel(const float* __restrict
         if (v > m) {
             s = s * expf(m - v) + 1.f;
             m = v;
-        } else {
+        } else if (v != NEG_INF) {          // -inf adds 0; with m = -inf too, exp(-inf - -inf) would be NaN
             s += expf(v - m);
         }
     }

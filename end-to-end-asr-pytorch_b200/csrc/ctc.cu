@@ -17,6 +17,7 @@
 // exp(lp) - exp(log sum(alpha*beta) + nll - lp)  (SURVEY.md F9).
 #include "common.cuh"
 #include "../../include/b200asr.h"
+#include "../../include/b200asr_debug.h"
 
 namespace b200asr {
 
@@ -30,7 +31,9 @@ __global__ void __launch_bounds__(256) log_softmax_fwd_kernel(const float* __res
     const float* xr = x + row * V;
     float m = NEG_INF, s = 0.f;
     int mi = 0x7fffffff;
-    if ((V & 3) == 0 && (reinterpret_cast<uintptr_t>(xr) & 15) == 0) {
+    // 128-bit loads and stores only when every row of x and y is 16-byte aligned (a contiguous view may start anywhere)
+    const bool vec4 = (V & 3) == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
+    if (vec4) {
         // 128-bit streaming, two independent loads in flight per lane, ONE rescale per 8 values (the running (max, sum)
         // pair is the only loop-carried dependency); the first index wins ties like torch.argmax
         const float4* x4 = reinterpret_cast<const float4*>(xr);
@@ -65,7 +68,7 @@ __global__ void __launch_bounds__(256) log_softmax_fwd_kernel(const float* __res
                 s = s * expf(m - v) + 1.f;  // m=-inf: s=0 -> 0*exp(-inf)=0
                 m = v;
                 mi = c;
-            } else {
+            } else if (v != NEG_INF) {      // -inf adds 0; with m = -inf too, exp(-inf - -inf) would be NaN
                 s += expf(v - m);
             }
         }
@@ -87,7 +90,7 @@ __global__ void __launch_bounds__(256) log_softmax_fwd_kernel(const float* __res
     const float L = M + logf(S);
     if (y == nullptr) {
         // statistics only (fused CTC head): the log-probs are never materialised
-    } else if ((V & 3) == 0) {
+    } else if (vec4) {
         const float4* x4 = reinterpret_cast<const float4*>(xr);
         float4* y4 = reinterpret_cast<float4*>(y + row * V);
         for (int c = lane; c < (V >> 2); c += 32) {
@@ -112,7 +115,8 @@ __global__ void __launch_bounds__(256) log_softmax_bwd_kernel(const float* __res
     const float* gr = g + row * V;
     const float* lr = lp + row * V;
     float s = 0.f;
-    if ((V & 3) == 0) {
+    if ((V & 3) == 0 &&
+        ((reinterpret_cast<uintptr_t>(lp) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0) {
         const float4* g4 = reinterpret_cast<const float4*>(gr);
         const float4* l4 = reinterpret_cast<const float4*>(lr);
         float4* d4 = reinterpret_cast<float4*>(dx + row * V);
@@ -536,7 +540,12 @@ __global__ void __launch_bounds__(CTC_GRAD_THREADS, 8) ctc_grad_kernel(CtcParams
     const int Lb = (int)(Lb64 < 0 ? 0 : (Lb64 > p.L_max ? p.L_max : Lb64));
     const int Sb = 2 * Lb + 1;
     const float nll = p.nll[b];
-    const float scale = (p.scale ? p.scale[b] : 1.f) * (p.upstream ? *p.upstream : 1.f);
+    // An utterance without any alignment (nll = +inf) gets ATen's value for zero_infinity=False: NaN at every element of
+    // its live frames (exp(lp) - exp(-inf + inf - lp)), so that the grad norm is NaN and the update is skipped.  A NaN
+    // scale makes phase 1 write exactly that; frames at t >= input_length keep their 0.
+    const bool infeasible = isinf(nll) && nll > 0.f;
+    const float scale = infeasible ? __int_as_float(0x7fc00000)
+                                   : (p.scale ? p.scale[b] : 1.f) * (p.upstream ? *p.upstream : 1.f);
     const bool vec4 = ((V & 3) == 0) && ((p.sb & 3) == 0) && ((p.st & 3) == 0) &&
                       ((reinterpret_cast<uintptr_t>(p.lp) | reinterpret_cast<uintptr_t>(p.grad)) & 15) == 0;
 
@@ -588,6 +597,7 @@ __global__ void __launch_bounds__(CTC_GRAD_THREADS, 8) ctc_grad_kernel(CtcParams
             for (int c = threadIdx.x; c < V; c += blockDim.x) gt[c] = live ? expf(lpt[c] - ls) * scale : 0.f;
         }
     }
+    if (infeasible) return;         // block-uniform; the gradient is NaN already (and alpha + beta is -inf everywhere)
     __syncthreads();
     // ---- phase 2: occupancy of the utterance's own classes.  One WARP per frame of the chunk (warp-synchronous: the
     // block-wide version spent its time in ~10 barriers per frame, which the other resident blocks had to cover)
@@ -697,6 +707,17 @@ static int ctc_launch_grad(const CtcParams& p, cudaStream_t stream) {
     return B200_OK;
 }
 
+// Lattice kernel for a padded target width: 1-4 = the warp kernel with that many extended-label positions per lane,
+// 5 = the block kernel with one position per thread, 6 = the block kernel with a strided loop over the positions.
+// The warp-synchronous kernel wins while a lane holds few positions (subword targets: S <= 128); for long character
+// targets one position per thread + a block barrier is faster (V = 31, L ~ 130), so those take the block kernel.
+static int ctc_variant(int L_max) {
+    const int S = 2 * L_max + 1;
+    const int need = (S + 31) / 32;            // extended-label positions per lane
+    if (need <= 4 && (size_t)CTC_WARPS * 2 * S * sizeof(float) <= 48 * 1024) return need;
+    return S <= 1024 ? 5 : 6;                  // the block kernel runs min(S, 1024) threads
+}
+
 static int ctc_fwd_bwd_impl(const float* log_probs, const float* row_lse, long long stride_b, long long stride_t,
                             const long long* targets, const long long* input_lengths,
                             const long long* target_lengths, int B, int T, int V, int L_max, int blank,
@@ -706,18 +727,16 @@ static int ctc_fwd_bwd_impl(const float* log_probs, const float* row_lse, long l
     const int rc = ctc_setup(p, log_probs, row_lse, stride_b, stride_t, targets, input_lengths, target_lengths, B, T, V,
                              L_max, blank, nll, grad_scale, nullptr, grad, workspace, workspace_bytes, "ctc_fwd_bwd");
     if (rc != B200_OK) return rc;
-    const int need = (p.S_max + 31) / 32;      // extended-label positions per lane
-    // The warp-synchronous kernel wins while a lane holds few positions (subword targets: S <= 128); for long
-    // character targets one position per thread + a block barrier is faster (V = 31, L ~ 130), so those
-    // take the block kernel.
-    if (need <= 4 && (size_t)CTC_WARPS * 2 * p.S_max * sizeof(float) <= 48 * 1024) {
-        if (need <= 1) launch_ctc_warp<1>(p, (cudaStream_t)stream);
-        else if (need <= 2) launch_ctc_warp<2>(p, (cudaStream_t)stream);
-        else if (need <= 3) launch_ctc_warp<3>(p, (cudaStream_t)stream);
+    const int variant = ctc_variant(L_max);
+    if (variant <= 4) {
+        if (variant == 1) launch_ctc_warp<1>(p, (cudaStream_t)stream);
+        else if (variant == 2) launch_ctc_warp<2>(p, (cudaStream_t)stream);
+        else if (variant == 3) launch_ctc_warp<3>(p, (cudaStream_t)stream);
         else launch_ctc_warp<4>(p, (cudaStream_t)stream);
         B200_LAUNCH_CHECK("ctc_alpha_beta_warp_kernel");
     } else {
-        // long targets: block-per-(utterance, direction) kernel with the lattice row in shared memory
+        // long targets: block-per-(utterance, direction) kernel with the lattice row in shared memory (one position per
+        // thread up to 1024 positions, variant 5; a strided loop over the positions beyond, variant 6)
         const size_t S = (size_t)p.S_max;
         int threads = (p.S_max + 31) / 32 * 32;
         if (threads > 1024) threads = 1024;
@@ -732,6 +751,8 @@ static int ctc_fwd_bwd_impl(const float* log_probs, const float* row_lse, long l
     if (grad) return ctc_launch_grad(p, (cudaStream_t)stream);
     return B200_OK;
 }
+
+extern "C" int b200asr_debug_ctc_variant(int L_max) { return L_max < 0 ? 0 : ctc_variant(L_max); }
 
 extern "C" int b200asr_ctc_fwd_bwd(const float* log_probs, long long stride_b, long long stride_t,
                                    const long long* targets, const long long* input_lengths,

@@ -81,7 +81,9 @@ B200ASR_API int b200asr_log_softmax_bwd(const float* log_probs, const float* gra
  * [B, L_max] zero padded int64; input_lengths / target_lengths [B] int64.  nll [B] out (per-utterance negative
  * log likelihood, +inf when infeasible).  If grad != NULL it receives, with the same strides as log_probs,
  * grad_scale[b] * (exp(lp) - exp(log sum_{s: l'_s = c} alpha_t(s) beta_t(s) + nll - lp)) for t < input_length
- * and 0 after it - ATen's convention (SURVEY.md F9).  grad_scale may be NULL (= 1).                         */
+ * and 0 after it - ATen's convention (SURVEY.md F9).  grad_scale may be NULL (= 1).  An infeasible utterance
+ * (nll = +inf) gets ATen's zero_infinity=False gradient: NaN at every element for t < input_length, 0 after it
+ * (all 0 when input_length is 0); the NaN grad norm then makes the fused update skip the step.               */
 B200ASR_API size_t b200asr_ctc_workspace_bytes(int B, int T, int L_max);
 B200ASR_API int b200asr_ctc_fwd_bwd(const float* log_probs, long long stride_b, long long stride_t, const long long* targets,
                         const long long* input_lengths, const long long* target_lengths, int B, int T, int V,

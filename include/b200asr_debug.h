@@ -16,6 +16,13 @@ B200ASR_API void b200asr_debug_set_lstm_trace(long long* device_buffer);
  * 1024 / 2048 = the other state-exchange protocol of the wgmma forward / backward kernel (flag + bulk copy <->
  * data-is-the-flag polling), 128 = trace the backward kernel; see tools/time_lstm.py. */
 B200ASR_API void b200asr_debug_set_lstm_mode(int mode);
+/* test: which alpha/beta lattice kernel b200asr_ctc_fwd_bwd(_logits) runs for a padded target width L_max: 1-4 = the
+ * warp kernel with that many extended-label positions per lane, 5 = the block kernel with one position per thread,
+ * 6 = the block kernel with a strided loop over the positions.  The dispatcher calls the same rule. */
+B200ASR_API int b200asr_debug_ctc_variant(int L_max);
+/* test: the minimum-blocks-per-SM instance (1 or 2) of the location-attention backward kernel that
+ * b200asr_locattn_bwd(_acc) launches for these sizes on the current device; 0 for bad sizes. */
+B200ASR_API int b200asr_debug_locattn_bwd_minb(int B, int T, int D, int E);
 
 #ifdef __cplusplus
 }
