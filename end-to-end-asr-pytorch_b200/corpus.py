@@ -41,3 +41,56 @@ class LibriDataset(Dataset):
 
     def __len__(self):
         return len(self.file_list)
+
+
+# Official LibriSpeech LM text (corpus/librispeech.py:9-12 in the reference): read line by line, encoded on the fly, and
+# the REMOVE_TOP_N_TXT longest lines dropped
+OFFICIAL_TXT_SRC = ["librispeech-lm-norm.txt"]
+REMOVE_TOP_N_TXT = 5000000
+
+
+class LibriTextDataset(Dataset):
+    """Sentences of LibriSpeech splits for the RNN LM (corpus/librispeech.py:64-122): transcripts found through the
+    `*.flac` files of a split, and/or the lines of librispeech-lm-norm.txt.  All sentences are sorted by length,
+    longest first (with the lm-norm file the length of the raw line, then the top REMOVE_TOP_N_TXT are dropped and
+    every sentence is encoded when first served).  Files are listed in sorted path order."""
+
+    def __init__(self, path, split, tokenizer, bucket_size):
+        self.path, self.bucket_size = path, bucket_size
+        self.encode_on_fly = False
+        files, sents = [], []
+        for s in split:
+            if s in OFFICIAL_TXT_SRC:
+                self.encode_on_fly = True
+                with open(Path(path, s), "r") as f:
+                    sents += f.readlines()
+            files += sorted(Path(path, s).rglob("*.flac"))
+        assert len(files) > 0 or len(sents) > 0, "No data found @ {}".format(path)
+        cache = {}
+        for f in files:
+            d = str(f.parent)
+            if d not in cache:
+                cache[d] = _transcripts(d)
+            sents.append(cache[d][f.name.split(".")[0]])
+        if self.encode_on_fly:
+            self.tokenizer = tokenizer
+            self.text = sents
+        else:
+            self.text = [tokenizer.encode(t) for t in sents]
+        self.text = sorted(self.text, reverse=True, key=len)
+        if self.encode_on_fly:
+            del self.text[:REMOVE_TOP_N_TXT]
+
+    def _item(self, i):
+        if self.encode_on_fly and type(self.text[i]) is str:
+            self.text[i] = self.tokenizer.encode(self.text[i])
+        return self.text[i]
+
+    def __getitem__(self, index):
+        if self.bucket_size > 1:
+            index = min(len(self.text) - self.bucket_size, index)
+            return [self._item(i) for i in range(index, index + self.bucket_size)]
+        return self._item(index)
+
+    def __len__(self):
+        return len(self.text)

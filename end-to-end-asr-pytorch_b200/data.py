@@ -156,3 +156,78 @@ def _data_msg(name, path, train_split, tr_set, dev_split, dv_set, batch_size, bu
             "           | Train sets = {}\t| Number of utts = {}".format(train_split, tr_set),
             "           | Dev sets = {}\t| Number of utts = {}".format(dev_split, dv_set),
             "           | Batch size = {}\t\t| Bucketing = {}".format(batch_size, bucketing)]
+
+
+# ---- text (RNN language model): src/data.py:57-73,109-134,183-202 -------------------------------------------------
+def collect_text_batch(batch, mode, vocab_size=None):
+    """[txt, ...] (or a bucket [[txt, ...]]) -> txt [B, L] int64, zero padded, in the dataset's order (longest first).
+    A train bucket whose first sentence is longer than HALF_BATCHSIZE_TEXT_LEN tokens is halved.  With `vocab_size`
+    every id is checked against [0, vocab_size) here, on the host, before anything reaches the device."""
+    if type(batch[0][0]) is list:
+        batch = batch[0]
+    if len(batch[0]) > HALF_BATCHSIZE_TEXT_LEN and mode == "train":
+        batch = batch[:len(batch) // 2]
+    text = [torch.LongTensor(b) for b in batch]
+    if vocab_size is not None:
+        for t in text:
+            if t.numel() and (int(t.min()) < 0 or int(t.max()) >= vocab_size):
+                raise ValueError("token id out of range [0, %d): min %d max %d" % (vocab_size, int(t.min()),
+                                                                                    int(t.max())))
+    return pad_sequence(text, batch_first=True)
+
+
+class SyntheticTextDataset(Dataset):
+    """Seeded sentences for tests and timing: lengths ~ U[min_len, max_len] tokens including <eos> = 1, ids in
+    [3, vocab_size), sorted longest first like LibriTextDataset; bucketed the same way."""
+
+    def __init__(self, vocab_size, n_sent, bucket_size, seed=0, min_len=2, max_len=40):
+        g = torch.Generator().manual_seed(seed)
+        lens = torch.randint(min_len, max_len + 1, (n_sent,), generator=g).tolist()
+        self.text = [torch.randint(3, vocab_size, (n - 1,), generator=g).tolist() + [1] for n in lens]
+        self.text = sorted(self.text, reverse=True, key=len)
+        self.bucket_size = bucket_size
+
+    def __getitem__(self, index):
+        if self.bucket_size > 1:
+            index = min(len(self.text) - self.bucket_size, index)
+            return self.text[index:index + self.bucket_size]
+        return self.text[index]
+
+    def __len__(self):
+        return len(self.text)
+
+
+def create_textset(tokenizer, train_split, dev_split, name, path, bucketing, batch_size, **extra):
+    """Same roles as src/data.py:109-134: (tr_set, dv_set, tr_loader_bs, dv_loader_bs, msg)."""
+    bucket_size = batch_size if bucketing else 1
+    tr_loader_bs = 1 if bucketing else batch_size
+    if name.lower() == "synthetic":
+        v = tokenizer.vocab_size
+        lo, hi = extra.get("min_len", 2), extra.get("max_len", 40)
+        dv_set = SyntheticTextDataset(v, extra.get("n_dev", 2 * batch_size), 1, seed=10 ** 6, min_len=lo, max_len=hi)
+        tr_set = SyntheticTextDataset(v, extra.get("n_sent", 16 * batch_size), bucket_size, seed=extra.get("seed", 0),
+                                      min_len=lo, max_len=hi)
+    elif name.lower() == "librispeech":
+        from .corpus import LibriTextDataset as Dataset_
+        dv_set = Dataset_(path, dev_split, tokenizer, 1)
+        tr_set = Dataset_(path, train_split, tokenizer, bucket_size)
+    else:
+        raise NotImplementedError(name)
+    msg = _data_msg(name, path, str(train_split), len(tr_set), str(dev_split), len(dv_set), batch_size, bucketing)
+    return tr_set, dv_set, tr_loader_bs, batch_size, msg
+
+
+def load_textset(n_jobs, use_gpu, pin_memory, corpus, text):
+    """Same signature and 5-tuple as src/data.py:183-202 (text stays in RAM: no loader workers, as there)."""
+    synthetic = corpus["name"].lower() == "synthetic"
+    tokenizer = _VocabOnly(corpus.get("vocab_size", 31)) if synthetic else load_text_encoder(**text)
+    tr_set, dv_set, tr_bs, dv_bs, msg = create_textset(tokenizer, **corpus)
+    V = tokenizer.vocab_size
+    tr_loader = DataLoader(tr_set, batch_size=tr_bs, shuffle=True, drop_last=True,
+                           collate_fn=partial(collect_text_batch, mode="train", vocab_size=V), num_workers=0,
+                           pin_memory=use_gpu)
+    dv_loader = DataLoader(dv_set, batch_size=dv_bs, shuffle=False, drop_last=False,
+                           collate_fn=partial(collect_text_batch, mode="dev", vocab_size=V), num_workers=0,
+                           pin_memory=pin_memory)
+    msg.append("I/O spec.  | Token type = {}\t| Vocab size = {}".format(tokenizer.token_type, V))
+    return tr_loader, dv_loader, V, tokenizer, msg

@@ -63,6 +63,8 @@ SIGNATURES = {
                                         c_int, c_int, _P, _P, _P, _P, _P]),
     "b200asr_attn_dvalue": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, c_int, _P]),
     "b200asr_ce_fwd_bwd": (c_int, [_P, _P, c_longlong, c_longlong, c_int, _P, _P, _P, _P]),
+    "b200asr_embedding_bwd_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "b200asr_embedding_bwd": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_size_t, _P]),
     "b200asr_gemm3x_supported": (c_int, [c_int, c_int, c_int]),
     "b200asr_gemm3x_tn": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     "b200asr_gemm3x_tn_ld": (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),

@@ -141,18 +141,24 @@ def gemm_nn(a, w, out=None, accumulate=False):
     return out
 
 
-def gemm_nt(a, b, M, N, T, batches=1, lda=None, a_bstride=0, ldb=None, b_bstride=0, b_shift=0, permute_rows=False):
-    """out[M,N] = sum over (batch, t) of a[batch, t, :M]^T b[batch, t + b_shift, :N]: the weight gradient dY^T . X.
-    `a` / `b` are tensors whose data pointer is element (0, 0, 0); pitches are in floats (default: dense [T, M] / [T, N])."""
+def gemm_nt(a, b, M, N, T, batches=1, lda=None, a_bstride=0, ldb=None, b_bstride=0, b_shift=0, permute_rows=False,
+            out=None, accumulate=False):
+    """out[M,N] (= or +=) sum over (batch, t) of a[batch, t, :M]^T b[batch, t + b_shift, :N]: the weight gradient
+    dY^T . X.  `a` / `b` are tensors whose data pointer is element (0, 0, 0); pitches are in floats (default: dense
+    [T, M] / [T, N]).  A given `out` must be a contiguous [M, N] fp32 tensor (e.g. a parameter's gradient view)."""
     lib = L.load()
     lda = M if lda is None else lda
     ldb = N if ldb is None else ldb
-    out = torch.empty((M, N), device=a.device, dtype=torch.float32)
+    if out is None:
+        out = torch.empty((M, N), device=a.device, dtype=torch.float32)
+        accumulate = False
+    assert out.is_contiguous() and out.dtype == torch.float32 and out.numel() == M * N
     ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
     ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
-    with L.timed("gemm3x_nt", 4 * (batches * T * (M + N) + M * N)):
+    with L.timed("gemm3x_nt", 4 * (batches * T * (M + N) + M * N * (2 if accumulate else 1))):
         L.check(lib.b200asr_gemm3x_nt(L.ptr(a), lda, a_bstride, 0, L.ptr(b), ldb, b_bstride, b_shift, L.ptr(out), M, N,
-                                      T, batches, N, 0, int(bool(permute_rows)), L.ptr(ws), ws_bytes, L.stream()),
+                                      T, batches, N, int(bool(accumulate)), int(bool(permute_rows)), L.ptr(ws),
+                                      ws_bytes, L.stream()),
                 "gemm3x_nt")
     return out
 
@@ -301,6 +307,9 @@ class BiLSTMFn(Function):
     @staticmethod
     def forward(ctx, x, ndir, *params):
         lib = L.load()
+        sink = None
+        if params and isinstance(params[-1], CStateSink):
+            sink, params = params[-1], params[:-1]
         assert len(params) == 4 * ndir
         Op, mm = _gemm_ops()
         x = _f32c(x)
@@ -333,8 +342,11 @@ class BiLSTMFn(Function):
         with L.timed("bilstm_fwd", ndir * (24 * B * H * T + 16 * H * H)):
             L.check(lib.b200asr_bilstm_fwd(L.ptr(gates), L.ptr(w_hh), L.ptr(cst), L.ptr(out), B, T, H, ndir,
                                            L.ptr(ws), ws_bytes, L.stream()), "bilstm_fwd")
+        if sink is not None:
+            sink.cstate = cst
         ctx.ndir = ndir
         ctx.dims = (B, T, I, H)
+        ctx.tail = (None,) if sink is not None else ()
         ctx.consumed = False
         ctx.save_for_backward(x, gates, cst, out, w_hh, *w_ih_p)
         return out
@@ -378,7 +390,7 @@ class BiLSTMFn(Function):
                 db = torch.empty((4 * H,), device=dev, dtype=torch.float32)
                 db.index_copy_(0, perm, g2.sum(0))
                 grads += [dw_ih, dw_hh, db, db.clone()]
-            return (dx2.view(B, T, I) if need_dx else None, None, *grads)
+            return (dx2.view(B, T, I) if need_dx else None, None, *grads, *ctx.tail)
         xs = Op(x.view(B * T, I))
         for d in range(ndir):
             dG = Op(gates[d].view(B * T, 4 * H))  # d(loss)/d(pre-activation), unit-major columns
@@ -400,11 +412,17 @@ class BiLSTMFn(Function):
             dw_hh.index_copy_(0, perm, mm(dG.t(), Op(hprev.view(B * T, H))))
             del dG, hprev
             grads += [dw_ih, dw_hh, db, db.clone()]
-        return (dx2.view(B, T, I) if need_dx else None, None, *grads)
+        return (dx2.view(B, T, I) if need_dx else None, None, *grads, *ctx.tail)
 
 
-def bilstm(x, lstm_params, ndir):
-    return BiLSTMFn.apply(x, ndir, *lstm_params)
+class CStateSink:
+    """Passed as the last argument of BiLSTMFn.apply: receives the layer's cell-state stash [ndir, B, T, H] (c after
+    every step), from which a caller reads the final cell state of each row."""
+    cstate = None
+
+
+def bilstm(x, lstm_params, ndir, sink=None):
+    return BiLSTMFn.apply(x, ndir, *lstm_params, *((sink,) if sink is not None else ()))
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -1013,3 +1031,94 @@ def linear3x(x, layer):
     if x.is_cuda and rows * layer.in_features * layer.out_features >= (1 << 24):
         return Linear3xFn.apply(x, layer.weight, layer.bias)
     return torch.nn.functional.linear(x, layer.weight, layer.bias)
+
+
+# ----------------------------------------------------------------------------------------------------------
+# RNN language model (src/lm.py): the V x E-sized gradients are added IN PLACE into the parameter's gradient - under
+# optim.Optimizer the `emb.weight` view of the flat gradient buffer, zeroed by pre_step - and the backward returns None
+# for the weight (the accumulator-node idea of AttnMemFn / DecWeightsFn).  Without a gradient buffer one zero [V, E]
+# tensor is allocated as `.grad` once.
+def _grad_view(p):
+    if p.grad is None:
+        p.grad = torch.zeros_like(p)
+    g = p.grad
+    if g.dtype != torch.float32 or not g.is_contiguous() or g.shape != p.shape:
+        raise L.B200AsrError("in-place gradient needs a contiguous fp32 .grad of the parameter's shape")
+    return g
+
+
+def embedding_bwd_(dW, ids, dy):
+    """dW[ids[n], :] += dy[n, :] in place (b200asr_embedding_bwd): deterministic, ids outside [0, V) skipped."""
+    lib = L.load()
+    V, E = dW.shape
+    ids = ids.reshape(-1).to(device=dW.device, dtype=torch.int64).contiguous()
+    dy = _f32c(dy.reshape(-1, E))
+    N = ids.numel()
+    if dy.shape[0] != N:
+        raise L.B200AsrError("embedding_bwd: %d ids but %d gradient rows" % (N, dy.shape[0]))
+    if not (dW.is_contiguous() and dW.dtype == torch.float32):
+        raise L.B200AsrError("embedding_bwd: dW must be a contiguous fp32 [V, E] tensor")
+    ws_bytes = lib.b200asr_embedding_bwd_workspace_bytes(N, V)
+    ws = torch.empty(max(ws_bytes, 16), device=dW.device, dtype=torch.uint8)
+    # algorithmic bytes: the ids and dY once, the touched rows of dW read and written (bounded by N rows)
+    with L.timed("embedding_bwd", 8 * N + 4 * N * E + 8 * min(N, V) * E):
+        L.check(lib.b200asr_embedding_bwd(L.ptr(ids), L.ptr(dy), N, V, E, L.ptr(dW), L.ptr(ws), ws_bytes, L.stream()),
+                "embedding_bwd")
+    return dW
+
+
+class EmbeddingFn(Function):
+    """nn.Embedding forward (ATen row gather, like the decoder's pre_embed); backward = embedding_bwd_ into
+    weight.grad in place, None returned for the weight."""
+
+    @staticmethod
+    def forward(ctx, ids, weight):
+        ctx.save_for_backward(ids)
+        ctx.weight = weight
+        return torch.nn.functional.embedding(ids, weight.detach())
+
+    @staticmethod
+    def backward(ctx, dy):
+        (ids,) = ctx.saved_tensors
+        if ctx.needs_input_grad[1]:
+            embedding_bwd_(_grad_view(ctx.weight), ids, dy)
+        return None, None
+
+
+def embedding(ids, weight):
+    return EmbeddingFn.apply(ids, weight)
+
+
+class TiedLinearFn(Function):
+    """y = x W^T without bias with W = emb.weight (src/lm.py:42, weight tying): the 3xTF32 GEMM of Linear3xFn; the
+    weight gradient dY^T . X is accumulated by the GEMM epilogue straight into weight.grad, where the embedding kernel
+    adds its part too - no second [V, E] tensor."""
+
+    @staticmethod
+    def forward(ctx, x, weight):
+        shp = x.shape
+        x2 = _f32c(x).reshape(-1, shp[-1])
+        w = weight.detach()
+        if not (_use_umma(x2.shape[1]) and w.shape[0] % 4 == 0):
+            raise L.B200AsrError("tied projection: E and V must be multiples of 4 for the tensor-core GEMM "
+                                 "(E=%d V=%d)" % (x2.shape[1], w.shape[0]))
+        y = gemm_tn(x2, w, w_lo=tf32_residual(w))
+        ctx.save_for_backward(x2)
+        ctx.weight = weight
+        ctx.shp = shp
+        return y.view(*shp[:-1], w.shape[0])
+
+    @staticmethod
+    def backward(ctx, gy):
+        (x2,) = ctx.saved_tensors
+        w = ctx.weight.detach()
+        V, E = w.shape
+        gy2 = _f32c(gy).reshape(-1, V)
+        dx = gemm_nn(gy2, w).view(ctx.shp) if ctx.needs_input_grad[0] else None
+        if ctx.needs_input_grad[1]:
+            gemm_nt(gy2, x2, V, E, gy2.shape[0], out=_grad_view(ctx.weight), accumulate=True)
+        return dx, None
+
+
+def tied_linear(x, weight):
+    return TiedLinearFn.apply(x, weight)

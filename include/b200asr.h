@@ -200,6 +200,18 @@ B200ASR_API int b200asr_ce_fwd_bwd(const float* logits, const long long* target,
                                    long long n_rows, int V, const float* grad_scale, float* row_loss,
                                    float* dlogits, b200asr_stream stream);
 
+/* ---- embedding backward: the gradient of the row gather  emb(x)  of the RNN language model (src/lm.py:17,32) ------
+ * replaces the backward of nn.Embedding there, which allocates and zero-fills a [V, E] tensor per step, scatters
+ * into it and has autograd add it into .grad:
+ *   dW[ids[n], :] += dY[n, :]   for n in [0, N), IN PLACE on an existing row-major [V, E] fp32 gradient.
+ * Deterministic, without float atomics: each touched row gets the sum of its occurrences taken in ascending n, added
+ * once onto its value; the result does not depend on the launch configuration.  Rows whose token does not occur are
+ * not touched, and ids outside [0, V) are skipped (neither read nor written).  dY is row-major [N, E];
+ * workspace >= b200asr_embedding_bwd_workspace_bytes(N, V) bytes, owned by the caller.                           */
+B200ASR_API size_t b200asr_embedding_bwd_workspace_bytes(int N, int V);
+B200ASR_API int b200asr_embedding_bwd(const long long* ids, const float* dY, int N, int V, int E, float* dW,
+                                      void* workspace, size_t workspace_bytes, b200asr_stream stream);
+
 /* ---- K16: gradient norm, clip and optimizer update on flat buffers (src/solver.py:84-89, src/optim.py) ----
  * grad_norm (device scalar) may be NULL (no clipping, no NaN skip); max_norm <= 0 disables clipping.          */
 B200ASR_API size_t b200asr_grad_norm_scratch_bytes(void);
