@@ -60,6 +60,7 @@ struct LstmParams {
     int flags;           // debug switches: bit 2 = first-generation MMA loops (every warp polls, compiler-pipelined),
                          // bit 3 = clock64 trace of the backward instead of the forward kernel
     int mma;             // 1: tensor-core (3xTF32 mma.sync) step GEMMs, see the *_mma kernels
+    int form;            // loop form of the mma.sync kernels, LstmVariant::form
 };
 
 #define LSTM_TRACE(slot) \
@@ -1054,10 +1055,10 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_fwd_mma_kernel(LstmPar
     }
     const int g = tid / LSTM_GTHREADS;
     if (g >= NH) return;
-    if (!(p.flags & 4) && H % 128 == 0)
+    if (p.form == 0)
         fwd_group_mma_v2(p, g, tid - g * LSTM_GTHREADS, dir, bg, ub, Wm, hs + (size_t)g * hs_half,
                          &full[g * LSTM_NCHUNK], &done[g], xb + (size_t)g * 2 * half_elems, turn);
-    else if (p.mma == 2)
+    else if (p.form == 2)
         fwd_group_mma<2>(p, g, tid - g * LSTM_GTHREADS, dir, bg, ub, Wm, hs + (size_t)g * hs_half,
                          &full[g * LSTM_NCHUNK], &done[g], xb + (size_t)g * 2 * half_elems, turn);
     else
@@ -1088,7 +1089,7 @@ __device__ __forceinline__ void bwd_group_mma(const LstmParams& p, int g, int gt
         it_ok[j] = it_in[j] && it_row[j] < p.Bend;
     }
     float dc_reg[2] = {0.f, 0.f};
-    const bool lead = (p.flags & 4) == 0;
+    const bool lead = p.form == 0;
     const bool trc = (g == 0 && gt == 0);
 
     for (int step = 0; step < T; ++step) {
@@ -1446,6 +1447,55 @@ static int make_plan(int B, int H, int ndir, Plan* out) {
     return 0;
 }
 
+// The step-kernel variant bilstm_run launches for a shape under the current debug mode.  bilstm_run makes its choice
+// through lstm_variant, so b200asr_debug_lstm_variant reports exactly what runs.
+struct LstmVariant {
+    int gen;      // 1: wgmma (lstm_umma.cu), 2: 3xTF32 mma.sync, 3: packed fp32 FMA
+    int UB;       // unit block
+    int UBP;      // template unit block: the wgmma forward's UB rounded up to 8 / 12 / 16; UB elsewhere
+    int poll;     // exchange protocol of the wgmma kernels: 1 = data-is-the-flag polling, 0 = flag + bulk copy
+    int strict;   // 1: formal acquire after the flag poll (wgmma flag protocol under debug mode 256)
+    int nsplit;   // consecutive launches over row blocks
+    int form;     // mma.sync forward: 0 = fwd_group_mma_v2, 1 / 2 = fwd_group_mma<1> / <2>;
+                  // mma.sync backward: 0 = one polling warp per group, 1 = every warp polls (flag bit 2); FMA: NH
+    int R;        // FMA register tile rows (4 or 8)
+    int vec;      // 1: the UB % 4 == 0 store path (wgmma forward publish, FMA backward scatter), 0: scalar stores
+};
+
+static int lstm_variant(int B, int H, int ndir, bool bwd, Plan* pl, LstmVariant* v) {
+    const int rc = make_plan(B, H, ndir, pl);
+    if (rc != 0) return rc;
+    *v = LstmVariant{};
+    const int uf = g_lstm_flags >> 4;
+    if (!bwd && g_lstm_mode == 0 && lstm_umma_fwd_variant(B, H, ndir, uf, &v->UB, &v->UBP, &v->poll, &v->nsplit)) {
+        v->gen = 1;
+        v->strict = (!v->poll && (uf & 1)) ? 1 : 0;
+        v->vec = (v->UB % 4 == 0) ? 1 : 0;
+        return 0;
+    }
+    // flag bit 5 (mode 512) toggles the backward between the wgmma kernel and the mma.sync generation
+    if (bwd && g_lstm_mode == 0 && (((g_lstm_flags & 32) != 0) != (LSTM_UMMA_BWD_DEFAULT != 0)) &&
+        lstm_umma_bwd_variant(B, H, ndir, uf, &v->UB, &v->poll, &v->nsplit)) {
+        v->gen = 1;
+        v->UBP = v->UB;
+        v->strict = (!v->poll && (uf & 1)) ? 1 : 0;
+        return 0;
+    }
+    v->UB = v->UBP = pl->UB;
+    v->nsplit = pl->nsplit;
+    if (pl->mma) {
+        v->gen = 2;
+        if (bwd) v->form = (g_lstm_flags & 4) ? 1 : 0;
+        else v->form = (!(g_lstm_flags & 4) && H % 128 == 0) ? 0 : pl->mma;
+    } else {
+        v->gen = 3;
+        v->form = pl->NH;
+        v->R = pl->R;
+        v->vec = (bwd && pl->UB % 4 == 0) ? 1 : 0;
+    }
+    return 0;
+}
+
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static long long* g_trace = nullptr;   // debug only: set through b200asr_debug_set_lstm_trace
 
@@ -1464,7 +1514,9 @@ extern "C" size_t b200asr_bilstm_workspace_bytes(int B, int T, int H, int ndir) 
 }
 
 extern "C" int b200asr_bilstm_uses_tcgen05(int B, int H, int ndir) {
-    return (g_lstm_mode == 0 && lstm_umma_fwd_supported(B, H, ndir)) ? 1 : 0;
+    Plan pl;
+    LstmVariant v;
+    return (lstm_variant(B, H, ndir, false, &pl, &v) == 0 && v.gen == 1) ? 1 : 0;
 }
 
 extern "C" int b200asr_bilstm_plan(int B, int H, int ndir, int* unit_block, int* batch_block, int* n_ctas) {
@@ -1490,15 +1542,14 @@ static int bilstm_run(bool bwd, float* gates, const float* w_hh, float* cstate, 
     B200_REQUIRE(B > 0 && T > 0 && H > 0 && (ndir == 1 || ndir == 2), "bilstm: bad sizes B=%d T=%d H=%d ndir=%d", B, T,
                  H, ndir);
     Plan pl;
-    B200_REQUIRE(make_plan(B, H, ndir, &pl) == 0,
+    LstmVariant v;
+    B200_REQUIRE(lstm_variant(B, H, ndir, bwd, &pl, &v) == 0,
                  "bilstm: no feasible decomposition for B=%d H=%d ndir=%d (H must be a multiple of 16)", B, H, ndir);
     B200_REQUIRE(workspace_bytes >= b200asr_bilstm_workspace_bytes(B, T, H, ndir), "bilstm: workspace too small");
-    if (!bwd && g_lstm_mode == 0 && lstm_umma_fwd_supported(B, H, ndir))
+    if (v.gen == 1 && !bwd)
         return lstm_umma_fwd(gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes,
                              (g_lstm_flags & 8) ? nullptr : g_trace, g_lstm_flags >> 4, stream);
-    // flag bit 5 (mode 512) toggles the backward between the wgmma kernel and the mma.sync generation
-    if (bwd && g_lstm_mode == 0 && (((g_lstm_flags & 32) != 0) != (LSTM_UMMA_BWD_DEFAULT != 0)) &&
-        lstm_umma_bwd_supported(B, H, ndir, g_lstm_flags >> 4))
+    if (v.gen == 1)
         return lstm_umma_bwd(gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes,
                              (g_lstm_flags & 8) ? g_trace : nullptr, g_lstm_flags >> 4, stream);
     unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
@@ -1520,7 +1571,7 @@ static int bilstm_run(bool bwd, float* gates, const float* w_hh, float* cstate, 
     LstmParams p;
     p.gates = gates; p.whh = packed; p.cst = cstate; p.out = out_or_dout; p.xbuf = xbuf; p.counters = counters;
     p.err_flag = err_flag; p.B = B; p.T = T; p.H = H; p.ndir = ndir; p.UB = pl.UB; p.Bc = pl.Bc; p.nub = pl.nub;
-    p.nbg = pl.nbg; p.NH = pl.NH; p.R = pl.R; p.mma = pl.mma; p.flags = g_lstm_flags;
+    p.nbg = pl.nbg; p.NH = pl.NH; p.R = pl.R; p.mma = pl.mma; p.form = v.form; p.flags = g_lstm_flags;
     p.trace = (bwd == ((g_lstm_flags & 8) != 0)) ? g_trace : nullptr;   // flag bit 3: trace the backward kernel
     const void* fn = !pl.mma ? (bwd ? (const void*)bilstm_bwd_kernel : (const void*)bilstm_fwd_kernel)
                              : (bwd ? (const void*)bilstm_bwd_mma_kernel : (const void*)bilstm_fwd_mma_kernel);
@@ -1540,6 +1591,17 @@ static int bilstm_run(bool bwd, float* gates, const float* w_hh, float* cstate, 
         count_launch();
     }
     return B200_OK;
+}
+
+extern "C" int b200asr_debug_lstm_variant(int B, int H, int ndir, int bwd, int* desc) {
+    Plan pl;
+    LstmVariant v;
+    if (B <= 0 || H <= 0 || (ndir != 1 && ndir != 2) || !desc) return -1;
+    const int rc = lstm_variant(B, H, ndir, bwd != 0, &pl, &v);
+    if (rc != 0) return rc;
+    const int d[9] = {v.gen, v.UB, v.UBP, v.poll, v.strict, v.nsplit, v.form, v.R, v.vec};
+    for (int i = 0; i < 9; ++i) desc[i] = d[i];
+    return 0;
 }
 
 extern "C" void b200asr_debug_set_lstm_trace(long long* device_buffer) { g_trace = device_buffer; }

@@ -66,7 +66,7 @@ __device__ __forceinline__ void red_relaxed_add_u32(unsigned* p, unsigned v) {
 // consumer polls the flag with RELAXED gpu-scope loads (served at the L2 coherence point) and then only ISSUES A BULK
 // COPY, whose reads are performed by the TMA unit at L2 - this thread never reads the data through its own L1, and the
 // copy is control-dependent on the polled value.  `strict` adds the formal acquire (one more L2 round trip) and the
-// generic->async proxy fence of the PTX memory model; both variants are tested.
+// generic->async proxy fence of the PTX memory model (debug mode 256); tests/test_gpu_lstm_variants.py runs both.
 __device__ __forceinline__ void ul_spin_until(const unsigned* ctr, unsigned target, int* err_flag, bool strict = false) {
     const long long t0 = clock64();
     while (ld_relaxed_u32(ctr) < target) {
@@ -479,13 +479,20 @@ __global__ void ul_pack_bwd_kernel(const float* __restrict__ w, uint8_t* __restr
 }
 
 
+__device__ __forceinline__ float add_ftz(float a, float b) {
+    float r;
+    asm("add.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+
 constexpr int ULB_EPI_WARPS = 16;
 constexpr int ULB_CTRL = 4;
 
 // POLL = the "data is the flag" exchange for the backward: every fp32 partial carries the parity of its buffer
 // generation in its least significant mantissa bit (2^-24 relative - below the resolution of the hi/lo product), the
 // destination polls its inbox IN GLOBAL MEMORY (L2) with relaxed loads until every word shows the expected tag and sums
-// straight from registers: no fence, no counter, no bulk copy, no shared-memory inbox.
+// straight from registers (flushing subnormals, so that a tagged zero adds nothing): no fence, no counter, no bulk
+// copy, no shared-memory inbox.
 template <int UB, bool POLL>
 __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm_bwd_umma_kernel(UlParams p) {
     constexpr int KS = (4 * UB) / 16;               // MMAs (k-steps of 16) per product and n-block
@@ -631,10 +638,13 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
                                     if ((__float_as_uint(v[j]) & 1u) == tag) pending &= ~(1u << j);
                                 }
                         }
+                        // flush-to-zero adds: a zero partial arrives with its tag as the smallest subnormal, and a
+                        // zero dout row must still get dG = 0 exactly (same FADD instruction, no extra work)
 #pragma unroll
                         for (int j = 0; j < 32; j += 4) {
                             if (j < nhere) {                          // nub is a multiple of 4 (ulb_plan)
-                                s0 += v[j]; s1 += v[j + 1]; s2 += v[j + 2]; s3 += v[j + 3];
+                                s0 = add_ftz(s0, v[j]); s1 = add_ftz(s1, v[j + 1]);
+                                s2 = add_ftz(s2, v[j + 2]); s3 = add_ftz(s3, v[j + 3]);
                             }
                         }
                     }
@@ -677,8 +687,10 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
                 float m = fmaxf(fmaxf(fabsf(dg.x), fabsf(dg.y)), fmaxf(fabsf(dg.z), fabsf(dg.w)));
 #pragma unroll
                 for (int o = 1; o < UB; o <<= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+                // e in [-113, 127] keeps sc = 2^(13-e) and its inverse 2^(e-13) normal: a tighter upper clamp would
+                // leave a row whose largest |dG| is >= 2^(clamp+3) above 65504 after scaling (hi = inf, lo = -inf)
                 int e = (int)((__float_as_uint(m) >> 23) & 0xffu) - 127;
-                e = e < -100 ? -100 : (e > 100 ? 100 : e);
+                e = e < -113 ? -113 : (e > 127 ? 127 : e);
                 const float sc = __uint_as_float((uint32_t)(127 + 13 - e) << 23);
                 // every warpgroup's MMAs of the previous step have read the A tiles (and the drains the row scales)
                 if (step > 0) mbar_wait(mma_done, (uint32_t)((step - 1) & 1));
@@ -882,17 +894,32 @@ int ul_launch_bwd(const UlbPlan& pl, UlParams p, const float* w_hh, cudaStream_t
 
 }  // namespace
 
+// flag bit 2 (debug mode 1024) / bit 3 (debug mode 2048) select the OTHER exchange protocol of the forward / backward
+static bool ul_poll(int flags) { return ((flags & 4) != 0) != (UL_POLL_FWD_DEFAULT != 0); }
 static bool ulb_poll(int flags) { return ((flags & 8) != 0) != (UL_POLL_BWD_DEFAULT != 0); }
 
-bool lstm_umma_bwd_supported(int B, int H, int ndir, int flags) {
+bool lstm_umma_bwd_variant(int B, int H, int ndir, int flags, int* ub, int* poll, int* nsplit) {
     UlbPlan pl;
-    return ulb_plan(B, H, ndir, ulb_poll(flags), &pl) == 0;
+    if (ulb_plan(B, H, ndir, ulb_poll(flags), &pl) != 0) return false;
+    *ub = pl.UB;
+    *poll = ulb_poll(flags) ? 1 : 0;
+    *nsplit = pl.nsplit;
+    return true;
+}
+
+bool lstm_umma_fwd_variant(int B, int H, int ndir, int flags, int* ub, int* ubp, int* poll, int* nsplit) {
+    UlPlan pl;
+    if (ul_plan(B, H, ndir, &pl) != 0) return false;
+    *ub = pl.UB;
+    *ubp = pl.UBp;
+    *poll = ul_poll(flags) ? 1 : 0;
+    *nsplit = pl.nsplit;
+    return true;
 }
 
 int lstm_umma_bwd(float* gates, const float* w_hh, const float* cstate, const float* dout, int B, int T, int H, int ndir,
                   void* workspace, size_t workspace_bytes, long long* trace, int flags, cudaStream_t stream) {
     UlbPlan pl;
-    // flag bit 3 (debug mode 2048) selects the OTHER exchange protocol than the default one
     const bool poll = ulb_poll(flags);
     B200_REQUIRE(ulb_plan(B, H, ndir, poll, &pl) == 0, "bilstm(umma bwd): unsupported shape B=%d H=%d ndir=%d", B, H, ndir);
     B200_REQUIRE(workspace_bytes >= lstm_umma_workspace_bytes(B, H, ndir), "bilstm(umma bwd): workspace too small");
@@ -909,11 +936,6 @@ int lstm_umma_bwd(float* gates, const float* w_hh, const float* cstate, const fl
     p.b0 = 0; p.Bend = B;
     if (pl.UB == 16) return poll ? ul_launch_bwd<16, true>(pl, p, w_hh, stream) : ul_launch_bwd<16, false>(pl, p, w_hh, stream);
     return poll ? ul_launch_bwd<8, true>(pl, p, w_hh, stream) : ul_launch_bwd<8, false>(pl, p, w_hh, stream);
-}
-
-bool lstm_umma_fwd_supported(int B, int H, int ndir) {
-    UlPlan pl;
-    return ul_plan(B, H, ndir, &pl) == 0;
 }
 
 size_t lstm_umma_workspace_bytes(int B, int H, int ndir) {
@@ -955,8 +977,7 @@ int lstm_umma_fwd(float* gates, const float* w_hh, float* cstate, float* out, in
     p.B = B; p.T = T; p.H = H; p.ndir = ndir; p.UB = pl.UB; p.nub = pl.nub; p.nbg = pl.nbg; p.NA = pl.NA;
     p.NC = pl.NA < UL_MAX_CTRL ? pl.NA : UL_MAX_CTRL;
     p.b0 = 0; p.Bend = B;
-    // flag bit 2 (debug mode 1024) selects the OTHER exchange protocol than the default one
-    const bool poll = ((flags & 4) != 0) != (UL_POLL_FWD_DEFAULT != 0);
+    const bool poll = ul_poll(flags);
     switch (pl.UBp) {
         case 8: return poll ? ul_launch_fwd<8, true>(pl, p, w_hh, stream) : ul_launch_fwd<8, false>(pl, p, w_hh, stream);
         case 12: return poll ? ul_launch_fwd<12, true>(pl, p, w_hh, stream) : ul_launch_fwd<12, false>(pl, p, w_hh, stream);

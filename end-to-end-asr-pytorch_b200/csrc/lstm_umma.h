@@ -5,8 +5,10 @@
 
 namespace b200asr {
 
-bool lstm_umma_fwd_supported(int B, int H, int ndir);
-bool lstm_umma_bwd_supported(int B, int H, int ndir, int flags);
+// The instance lstm_umma_fwd / lstm_umma_bwd launch for these sizes and flags: unit block, template unit block,
+// exchange protocol (1 = data-is-the-flag polling, 0 = flag + bulk copy) and number of launches.  false: no plan.
+bool lstm_umma_fwd_variant(int B, int H, int ndir, int flags, int* ub, int* ubp, int* poll, int* nsplit);
+bool lstm_umma_bwd_variant(int B, int H, int ndir, int flags, int* ub, int* poll, int* nsplit);
 int lstm_umma_bwd(float* gates, const float* w_hh, const float* cstate, const float* dout, int B, int T, int H, int ndir,
                   void* workspace, size_t workspace_bytes, long long* trace, int flags, cudaStream_t stream);
 size_t lstm_umma_workspace_bytes(int B, int H, int ndir);

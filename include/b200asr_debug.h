@@ -16,6 +16,14 @@ B200ASR_API void b200asr_debug_set_lstm_trace(long long* device_buffer);
  * 1024 / 2048 = the other state-exchange protocol of the wgmma forward / backward kernel (flag + bulk copy <->
  * data-is-the-flag polling), 128 = trace the backward kernel; see tools/time_lstm.py. */
 B200ASR_API void b200asr_debug_set_lstm_mode(int mode);
+/* test: the step-kernel variant b200asr_bilstm_fwd (bwd = 0) / _bwd (bwd = 1) runs for these sizes under the current
+ * lstm mode on the current device (132 SMs / 232448 B of shared memory without one).  Fills desc[9] =
+ * {generation (1 wgmma, 2 mma.sync 3xTF32, 3 fp32 FMA), unit block UB, template unit block (UBP of the wgmma forward,
+ *  else UB), exchange protocol (1 data-is-the-flag polling, 0 flag + bulk copy), strict acquire, nsplit (launches),
+ *  loop form (mma.sync forward 0 = v2, 1 / 2 = fwd_group_mma<1> / <2>; mma.sync backward 0 = one polling warp, 1 =
+ *  every warp polls; FMA: halves NH), FMA register-tile rows R, vectorised UB % 4 == 0 stores}.  Returns 0, or < 0
+ * when the shape has no plan.  The dispatcher makes its choice through the same function. */
+B200ASR_API int b200asr_debug_lstm_variant(int B, int H, int ndir, int bwd, int* desc);
 /* test: which alpha/beta lattice kernel b200asr_ctc_fwd_bwd(_logits) runs for a padded target width L_max: 1-4 = the
  * warp kernel with that many extended-label positions per lane, 5 = the block kernel with one position per thread,
  * 6 = the block kernel with a strided loop over the positions.  The dispatcher calls the same rule. */

@@ -7,7 +7,7 @@ import torch.nn.functional as F
 
 from conftest import load_golden, rel_err, scaled_err
 from oracle import oracle_np as onp
-from oracle import ref_port
+from oracle import lstm_ref, ref_port
 from oracle.make_golden import AUDIO_CFG
 
 pytestmark = pytest.mark.gpu
@@ -300,11 +300,20 @@ def test_bilstm_backward_generation_toggle(pkg, B, T, I, H, bidir):
 
 
 @pytest.mark.parametrize("B,T,I,H,bidir", [(64, 10, 120, 512, True), (32, 11, 24, 640, True), (40, 9, 16, 512, False),
-                                           (8, 13, 40, 320, True), (64, 300, 64, 512, True)])
+                                           (8, 13, 40, 320, True), (64, 300, 64, 512, True), (64, 11, 24, 256, True),
+                                           (64, 11, 24, 384, True)])
 def test_bilstm_exchange_protocol_toggle(pkg, B, T, I, H, bidir):
     """Mode flags 1024 (forward) / 2048 (backward) select the OTHER state-exchange protocol of the wgmma kernels than
-    the default one (data-is-the-flag polling <-> fence + counter + bulk copy): both stay parity-tested."""
+    the default one (data-is-the-flag polling <-> fence + counter + bulk copy).  The flag-protocol backward keeps an
+    inbox of 32 x H floats in shared memory, so it has a plan only at H = 256, 384 and 512; at H = 640 and at
+    H = 320 the mode runs the backward of the other generation (asserted through the variant query).
+    tests/test_gpu_lstm_variants.py checks every protocol per batch row against float64."""
     lib = pkg.load_library()
+    ndir = 2 if bidir else 1
+    fwd = lstm_ref.variant(lib, B, H, ndir, False, 1024 + 2048)
+    bwd = lstm_ref.variant(lib, B, H, ndir, True, 1024 + 2048)
+    assert fwd["gen"] == 1 and fwd["poll"] == 1
+    assert (bwd["gen"] == 1 and bwd["poll"] == 0) == (H in (256, 384, 512)), bwd
     lib.b200asr_debug_set_lstm_mode(1024 + 2048)
     try:
         _check_bilstm(pkg, B, T, I, H, bidir, wtol=2e-4 if T > 100 else 1e-4)
