@@ -44,6 +44,7 @@
 // 4096 bytes each (a TMA box {32 columns, 32 rows}); A's boxes with the 128-byte swizzle (see AFragAddr), B's
 // without (the transposing pass reads one k row of 32 columns per warp load).
 #include <cuda.h>
+#include <cuda_fp16.h>
 #include <stdlib.h>
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -236,6 +237,41 @@ __device__ __forceinline__ void mma_chunk(float (&d)[64], int i0, const uint8_t*
     if (lane == 0) g_arrive(&empty[(i0 + LEN - 1) % L::STAGES]);
 }
 
+// Epilogue of a consumer thread: its accumulator fragment (tile rows row0 / row1, columns n0 + 8 gq + 2 (lane % 4) + {0,1})
+// -> C (+ bias, + C when accumulating, rows through the gate permutation when perm), or -> its split-K partial tile.
+__device__ __forceinline__ void store_acc(const float (&acc)[64], const float* bias_in, float* C, float* partial, int M,
+                                          int N, int ldc_in, int accumulate_in, int perm, int row0, int row1, int n0,
+                                          int lane) {
+    const bool to_partial = gridDim.z > 1;
+    float* Cb = to_partial ? partial + (size_t)blockIdx.z * M * N : C;
+    const int ldc = to_partial ? N : ldc_in;
+    const float* bias = to_partial ? nullptr : bias_in;
+    const int accumulate = to_partial ? 0 : accumulate_in;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int row = h ? row1 : row0;
+        if (row >= M) continue;
+        const int orow = (!to_partial && perm) ? (row & 3) * (M >> 2) + (row >> 2) : row;
+        float* crow = Cb + (size_t)orow * ldc;
+        const bool vec = ((ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(Cb) & 7) == 0);
+#pragma unroll
+        for (int gq = 0; gq < 16; ++gq) {
+            const int n = n0 + 8 * gq + 2 * (lane & 3);
+            float o0 = acc[4 * gq + 2 * h], o1 = acc[4 * gq + 2 * h + 1];
+            if (bias && n < N) o0 += bias[n];
+            if (bias && n + 1 < N) o1 += bias[n + 1];
+            if (vec && n + 1 < N) {
+                float2* p2 = reinterpret_cast<float2*>(crow + n);
+                if (accumulate) { const float2 old = *p2; o0 += old.x; o1 += old.y; }
+                *p2 = make_float2(o0, o1);
+            } else {
+                if (n < N) crow[n] = accumulate ? crow[n] + o0 : o0;
+                if (n + 1 < N) crow[n + 1] = accumulate ? crow[n + 1] + o1 : o1;
+            }
+        }
+    }
+}
+
 // B_PRE: the residual of a K-major B comes from a pre-computed residual matrix (same shape / layout: the weights, split
 // once per step by b200asr_tf32_residual) through its own tensor map.  An MN-major B goes through the transposing
 // pass, which makes its residual in the same sweep.
@@ -329,35 +365,8 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
 #pragma unroll
             for (int e = 0; e < 64; ++e) acc[e] += d[e];            // IEEE-add the chunk
         }
-        // ---------------------------------------------------------------- epilogue: registers -> C
-        const bool to_partial = gridDim.z > 1;
-        float* Cb = to_partial ? g.partial + (size_t)blockIdx.z * M * N : g.C;
-        const int ldc = to_partial ? N : g.ldc;
-        const float* bias = to_partial ? nullptr : g.bias;
-        const int accumulate = to_partial ? 0 : g.accumulate;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int row = m0 + (A_MN ? mn_row(r0 + 8 * h) : r0 + 8 * h);
-            if (row >= M) continue;
-            const int orow = (!to_partial && g.perm) ? (row & 3) * (M >> 2) + (row >> 2) : row;
-            float* crow = Cb + (size_t)orow * ldc;
-            const bool vec = ((ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(Cb) & 7) == 0);
-#pragma unroll
-            for (int gq = 0; gq < 16; ++gq) {
-                const int n = n0 + 8 * gq + 2 * (lane & 3);
-                float o0 = acc[4 * gq + 2 * h], o1 = acc[4 * gq + 2 * h + 1];
-                if (bias && n < N) o0 += bias[n];
-                if (bias && n + 1 < N) o1 += bias[n + 1];
-                if (vec && n + 1 < N) {
-                    float2* p2 = reinterpret_cast<float2*>(crow + n);
-                    if (accumulate) { const float2 old = *p2; o0 += old.x; o1 += old.y; }
-                    *p2 = make_float2(o0, o1);
-                } else {
-                    if (n < N) crow[n] = accumulate ? crow[n] + o0 : o0;
-                    if (n + 1 < N) crow[n + 1] = accumulate ? crow[n + 1] + o1 : o1;
-                }
-            }
-        }
+        store_acc(acc, g.bias, g.C, g.partial, M, N, g.ldc, g.accumulate, g.perm,
+                  m0 + (A_MN ? mn_row(r0) : r0), m0 + (A_MN ? mn_row(r0 + 8) : r0 + 8), n0, lane);
     }
 }
 
@@ -514,6 +523,231 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mb, GemmArgs g, void* ws, s
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// f16x3: the LSTM layer contractions on scaled fp16 hi/lo images (DESIGN.md 2.2).  An operand X[outer][k] (k = the
+// contraction index) is stored as two K-major fp16 images [outer][Kp] (Kp = K rounded up to F_CK, zero-filled) and one
+// power-of-two scale per (outer index, chunk of F_CK k): s = 2^e brings the chunk's largest magnitude to [2^13, 2^14),
+//   hi = f16_rn(x s),  lo = f16_rn(x s - hi),  sinv[chunk][outer] = 2^-e.
+// x s is exact (power of two), |lo| <= 4 and lo stays an fp16 normal down to 2^-28 of the chunk maximum, so hi + lo
+// carries x to ~2^-24 of its chunk maximum with one fp32 accumulator (no x2048 lo and cross-term accumulator needed).
+// Per K block of 64 k each consumer warpgroup issues A_hi.B_hi + A_hi.B_lo + A_lo.B_hi (m64n128k16, both operands
+// from shared memory) into d; the accumulation chunk is the scale chunk, and its fold  acc += d sa[m] sb[n]  is exact
+// (powers of two).  Weight-gradient forms get their operands transposed by the split pass (f16_split_cols_kernel),
+// so every GEMM is the same K-major x K-major kernel.
+// Non-finite values: the chunk maximum is an integer max over the magnitude bit patterns, so a NaN (bits above Inf)
+// or an Inf is seen (fmaxf would drop a NaN); such a chunk gets scale 1, its NaN / Inf reaches hi or lo and poisons
+// exactly the outputs of its outer index, as in an fp32 GEMM (finite values of that chunk that overflow fp16 only
+// touch the same, already poisoned, outputs).  An all-zero chunk gets scale 1.
+constexpr int F_BK = 64;                  // fp16 k per K block: one 128-byte swizzle row
+constexpr int F_CK = 128;                 // k per scale chunk = per accumulation chunk
+constexpr int F_CH = F_CK / F_BK;         // K blocks per chunk
+constexpr int F_TILE = G_BM * F_BK * 2;   // 16 KB: one image tile (G_BM == G_BN)
+constexpr int F_STAGE = 4 * F_TILE;       // A hi | A lo | B hi | B lo
+constexpr int F_STAGES = 3;               // 192 KB
+
+struct F16Args {
+    const float* bias;
+    const float* sa;       // inverse scales of A [Kp / F_CK][M]
+    const float* sb;       // inverse scales of B [Kp / F_CK][N]
+    float* C;
+    float* partial;        // [nsplit][M][N] when nsplit > 1
+    int M, N, ldc, accumulate, perm;
+    int KB, kb_per_split;  // K blocks of F_BK, both multiples of F_CH
+};
+
+// floor(log2) of the largest magnitude (bit pattern, sign cleared) -> scale exponent, clamped so that 2^e and 2^-e
+// are fp32 normals
+__device__ __forceinline__ int f16_scale_exp(uint32_t amax) {
+    if (amax == 0u || amax >= 0x7f800000u) return 0;
+    const int E = amax >= 0x00800000u ? (int)(amax >> 23) - 127 : (31 - __clz((int)amax)) - 149;
+    return min(126, max(-126, 13 - E));
+}
+__device__ __forceinline__ float pow2f(int e) { return __uint_as_float((uint32_t)(127 + e) << 23); }
+__device__ __forceinline__ uint32_t abs_bits(float x) { return __float_as_uint(x) & 0x7fffffffu; }
+__device__ __forceinline__ void f16_split2(float x0, float x1, float s, __half2& hi, __half2& lo) {
+    const float y0 = x0 * s, y1 = x1 * s;
+    hi = __floats2half2_rn(y0, y1);
+    lo = __floats2half2_rn(y0 - __low2float(hi), y1 - __high2float(hi));
+}
+
+// K-major operand x[row][k] (pitch ld floats): one warp per (row, chunk), 4 k per lane
+__global__ void __launch_bounds__(256) f16_split_rows_kernel(const float* __restrict__ x, long long ld, int rows, int K,
+                                                             int Kp, __half* __restrict__ hi, __half* __restrict__ lo,
+                                                             float* __restrict__ sinv) {
+    const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, c = blockIdx.y;
+    if (row >= rows) return;
+    const int k = c * F_CK + 4 * lane;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (k < K) v = *reinterpret_cast<const float4*>(x + (size_t)row * ld + k);      // K % 4 == 0
+    const uint32_t a = __reduce_max_sync(0xffffffffu, max(max(abs_bits(v.x), abs_bits(v.y)), max(abs_bits(v.z), abs_bits(v.w))));
+    const int e = f16_scale_exp(a);
+    const float s = pow2f(e);
+    __half2 h[2], l[2];
+    f16_split2(v.x, v.y, s, h[0], l[0]);
+    f16_split2(v.z, v.w, s, h[1], l[1]);
+    const size_t o = (size_t)row * Kp + k;
+    *reinterpret_cast<uint2*>(hi + o) = *reinterpret_cast<const uint2*>(h);
+    *reinterpret_cast<uint2*>(lo + o) = *reinterpret_cast<const uint2*>(l);
+    if (lane == 0) sinv[(size_t)c * rows + row] = pow2f(-e);
+}
+
+// MN-major operand -> transposed image [col][r], r = b T + t over the contraction rows, element x[b bstride + (t + shift)
+// ld + col] (zero outside [0, T): the h_prev of a direction, shifted per utterance).  One CTA per (chunk of F_CK rows,
+// 64 columns) through shared memory; warp w then writes columns 8w .. 8w + 7, one 256-byte image row per column.
+__global__ void __launch_bounds__(256) f16_split_cols_kernel(const float* __restrict__ x, long long ld, long long bstride,
+                                                             int shift, int T, int R, int cols, int Rp,
+                                                             __half* __restrict__ hi, __half* __restrict__ lo,
+                                                             float* __restrict__ sinv) {
+    __shared__ float tile[F_CK][65];
+    const int r0 = blockIdx.y * F_CK, c0 = blockIdx.x * 64, tid = threadIdx.x;
+    const int cq = 4 * (tid & 15);
+#pragma unroll
+    for (int i = 0; i < F_CK / 16; ++i) {
+        const int rr = (tid >> 4) + 16 * i, r = r0 + rr;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (r < R && c0 + cq < cols) {                  // cols % 4 == 0
+            const int b = r / T, t = r - b * T + shift;
+            if (t >= 0 && t < T) v = *reinterpret_cast<const float4*>(x + b * bstride + (long long)t * ld + c0 + cq);
+        }
+        tile[rr][cq] = v.x; tile[rr][cq + 1] = v.y; tile[rr][cq + 2] = v.z; tile[rr][cq + 3] = v.w;
+    }
+    __syncthreads();
+    const int warp = tid >> 5, lane = tid & 31;
+    for (int j = 0; j < 8; ++j) {
+        const int cc = 8 * warp + j, col = c0 + cc;
+        if (col >= cols) break;
+        const float v0 = tile[2 * lane][cc], v1 = tile[2 * lane + 1][cc];
+        const float v2 = tile[64 + 2 * lane][cc], v3 = tile[65 + 2 * lane][cc];
+        const uint32_t a = __reduce_max_sync(0xffffffffu, max(max(abs_bits(v0), abs_bits(v1)), max(abs_bits(v2), abs_bits(v3))));
+        const int e = f16_scale_exp(a);
+        const float s = pow2f(e);
+        __half2 h0, l0, h1, l1;
+        f16_split2(v0, v1, s, h0, l0);
+        f16_split2(v2, v3, s, h1, l1);
+        const size_t o = (size_t)col * Rp + r0 + 2 * lane;
+        *reinterpret_cast<__half2*>(hi + o) = h0;
+        *reinterpret_cast<__half2*>(hi + o + 64) = h1;
+        *reinterpret_cast<__half2*>(lo + o) = l0;
+        *reinterpret_cast<__half2*>(lo + o + 64) = l1;
+        if (lane == 0) sinv[(size_t)blockIdx.y * cols + col] = pow2f(-e);
+    }
+}
+
+// One accumulation chunk (F_CH K blocks, starting at block i0 of the slice) into d (overwritten): block j + 1 is issued
+// before block j is waited for, the wait that retires a block releases its stage, the chunk ends in the only drain.
+__device__ __forceinline__ void f16_chunk(float (&d)[64], int i0, const uint8_t* smem, uint64_t* full, uint64_t* empty,
+                                          uint32_t a_off, int lane) {
+#pragma unroll
+    for (int j = 0; j < F_CH; ++j) {
+        const int i = i0 + j, s = i % F_STAGES;
+        mbar_wait(&full[s], (uint32_t)((i / F_STAGES) & 1));
+        const uint32_t st = smem_u32(smem + s * F_STAGE);
+        const uint32_t ahi = st + a_off, alo = ahi + F_TILE, bhi = st + 2 * F_TILE, blo = st + 3 * F_TILE;
+        wgmma::fence_operand(d);
+        wgmma::fence();
+#pragma unroll
+        for (int k = 0; k < F_BK / 16; ++k) {
+            const uint64_t dah = wgmma::desc_k_sw128(ahi + 32 * k), dbh = wgmma::desc_k_sw128(bhi + 32 * k);
+            wgmma::mma_f16_n128(d, dah, dbh, (j | k) != 0);
+            wgmma::mma_f16_n128(d, dah, wgmma::desc_k_sw128(blo + 32 * k), 1);
+            wgmma::mma_f16_n128(d, wgmma::desc_k_sw128(alo + 32 * k), dbh, 1);
+        }
+        wgmma::commit_group();
+        if (j + 1 < F_CH) wgmma::wait_group<1>();
+        else wgmma::wait_all();
+        if (lane == 0 && j > 0) g_arrive(&empty[(i - 1) % F_STAGES]);
+    }
+    wgmma::fence_operand(d);
+    if (lane == 0) g_arrive(&empty[(i0 + F_CH - 1) % F_STAGES]);
+}
+
+// C[M,N] (+)= sum_k A[m][k] B[n][k] (+ bias) on f16x3 images; 128 x 128 tile per CTA (x split-K slices), warp 0 lane 0
+// issues the TMA loads of the four image tiles, warpgroups 1 and 2 compute 64 rows each.
+__global__ void __launch_bounds__(G_THREADS, 1)
+gemm_f16x3_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constant__ CUtensorMap map_alo,
+                  const __grid_constant__ CUtensorMap map_bhi, const __grid_constant__ CUtensorMap map_blo,
+                  const F16Args g) {
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + F_STAGES * F_STAGE);
+    uint64_t* empty = full + F_STAGES;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int m0 = blockIdx.y * G_BM, n0 = blockIdx.x * G_BN;
+    const int kb0 = blockIdx.z * g.kb_per_split;
+    auto slice_blocks = [&]() { return min(g.KB, kb0 + g.kb_per_split) - kb0; };
+    if (tid == 0) {
+        for (int s = 0; s < F_STAGES; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], G_CONSUMERS / 32);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+
+    if (warp < 4) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(G_PRODUCER_REGS) : "memory");
+        if (warp == 0 && lane == 0) {
+            const int nkb = slice_blocks();
+            for (int i = 0; i < nkb; ++i) {
+                const int s = i % F_STAGES, k = (kb0 + i) * F_BK;
+                if (i >= F_STAGES) mbar_wait(&empty[s], (uint32_t)(((i / F_STAGES) - 1) & 1));
+                uint8_t* st = smem + s * F_STAGE;
+                mbar_expect_tx(&full[s], 4 * F_TILE);
+                tma_load_2d(st, &map_ahi, k, m0, &full[s]);
+                tma_load_2d(st + F_TILE, &map_alo, k, m0, &full[s]);
+                tma_load_2d(st + 2 * F_TILE, &map_bhi, k, n0, &full[s]);
+                tma_load_2d(st + 3 * F_TILE, &map_blo, k, n0, &full[s]);
+            }
+        }
+    } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(G_CONSUMER_REGS) : "memory");
+        const int nkb = slice_blocks();
+        const int wg = (warp >> 2) - 1;
+        const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+        const int row0 = m0 + r0, row1 = row0 + 8;
+        const int M = g.M, N = g.N;
+        float acc[64], d[64];
+#pragma unroll
+        for (int e = 0; e < 64; ++e) acc[e] = 0.f;
+        for (int i = 0; i < nkb; i += F_CH) {
+            // this chunk's inverse scales, loaded before its MMAs are issued (rows / columns beyond the matrix: 0)
+            const size_t c = (size_t)((kb0 + i) / F_CH);
+            const float sa0 = row0 < M ? g.sa[c * M + row0] : 0.f, sa1 = row1 < M ? g.sa[c * M + row1] : 0.f;
+            float sb[32];
+#pragma unroll
+            for (int gq = 0; gq < 16; ++gq) {
+                const int n = n0 + 8 * gq + 2 * (lane & 3);
+                sb[2 * gq] = n < N ? g.sb[c * N + n] : 0.f;
+                sb[2 * gq + 1] = n + 1 < N ? g.sb[c * N + n + 1] : 0.f;
+            }
+            f16_chunk(d, i, smem, full, empty, (uint32_t)(wg * 64 * 128), lane);
+#pragma unroll
+            for (int gq = 0; gq < 16; ++gq) {
+                acc[4 * gq] += d[4 * gq] * sa0 * sb[2 * gq];
+                acc[4 * gq + 1] += d[4 * gq + 1] * sa0 * sb[2 * gq + 1];
+                acc[4 * gq + 2] += d[4 * gq + 2] * sa1 * sb[2 * gq];
+                acc[4 * gq + 3] += d[4 * gq + 3] * sa1 * sb[2 * gq + 1];
+            }
+        }
+        store_acc(acc, g.bias, g.C, g.partial, M, N, g.ldc, g.accumulate, g.perm, row0, row1, n0, lane);
+    }
+}
+
+// fp16 image [rows][Kp] -> 2-D tensor map with boxes of F_BK (K) x 128 rows, 128-byte swizzle
+int make_map_f16(CUtensorMap* map, const void* ptr, int rows, int Kp) {
+    EncodeTiledFn enc = encode_fn();
+    B200_REQUIRE(enc != nullptr, "gemm: cuTensorMapEncodeTiled is not available from this driver");
+    const cuuint64_t dims[2] = {(cuuint64_t)Kp, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)Kp * 2};
+    const cuuint32_t box[2] = {(cuuint32_t)F_BK, (cuuint32_t)G_BM};
+    const cuuint32_t estr[2] = {1, 1};
+    const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    B200_REQUIRE(r == CUDA_SUCCESS, "gemm_f16x3: cuTensorMapEncodeTiled failed (%d) for a [%d x %d] image", (int)r, rows,
+                 Kp);
+    return B200_OK;
+}
+
 }  // namespace
 }  // namespace b200asr
 
@@ -656,3 +890,77 @@ extern "C" int b200asr_gemm3x_tn_pre2(const float* A, const float* A_lo, int lda
     return gemm3x_tn_impl(A, lda, B, bias, C, M, N, K, ldc, accumulate, workspace, workspace_bytes, stream, B_lo, A_lo);
 }
 
+
+extern "C" int b200asr_f16x3_padded_k(int K) { return K > 0 ? (K + F_CK - 1) / F_CK * F_CK : 0; }
+
+extern "C" int b200asr_f16x3_split_rows(const float* x, long long ld, int rows, int K, void* hi, void* lo, float* sinv,
+                                        b200asr_stream stream) {
+    B200_REQUIRE(x && hi && lo && sinv, "f16x3_split_rows: null pointer");
+    B200_REQUIRE(rows > 0 && K > 0 && (K % 4) == 0 && ld >= K && (ld % 4) == 0 && aligned16(x),
+                 "f16x3_split_rows: needs K %% 4 == 0, a pitch that is a multiple of 4 floats, 16-byte alignment "
+                 "(rows %d K %d ld %lld)", rows, K, ld);
+    const int Kp = b200asr_f16x3_padded_k(K);
+    dim3 grid((rows + 7) / 8, Kp / F_CK);
+    f16_split_rows_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ld, rows, K, Kp, (__half*)hi, (__half*)lo, sinv);
+    B200_LAUNCH_CHECK("f16_split_rows_kernel");
+    return B200_OK;
+}
+
+extern "C" int b200asr_f16x3_split_cols(const float* x, long long ld, long long bstride, int shift, int T, int batches,
+                                        int cols, void* hi, void* lo, float* sinv, b200asr_stream stream) {
+    B200_REQUIRE(x && hi && lo && sinv, "f16x3_split_cols: null pointer");
+    B200_REQUIRE(T > 0 && batches > 0 && cols > 0 && (cols % 4) == 0 && ld >= cols && (ld % 4) == 0 &&
+                     (bstride % 4) == 0 && (batches == 1 || bstride >= (long long)T * ld) && aligned16(x),
+                 "f16x3_split_cols: needs cols %% 4 == 0, pitches that are multiples of 4 floats, 16-byte alignment "
+                 "(cols %d ld %lld bstride %lld)", cols, ld, bstride);
+    B200_REQUIRE((long long)T * batches < (1LL << 31) - F_CK, "f16x3_split_cols: too many rows");
+    const int R = T * batches, Rp = b200asr_f16x3_padded_k(R);
+    dim3 grid((cols + 63) / 64, Rp / F_CK);
+    f16_split_cols_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ld, bstride, shift, T, R, cols, Rp, (__half*)hi,
+                                                                  (__half*)lo, sinv);
+    B200_LAUNCH_CHECK("f16_split_cols_kernel");
+    return B200_OK;
+}
+
+extern "C" int b200asr_gemm_f16x3(const void* a_hi, const void* a_lo, const float* a_sinv, const void* b_hi,
+                                  const void* b_lo, const float* b_sinv, const float* bias, float* C, int M, int N,
+                                  int Kp, int ldc, int accumulate, int permute_rows, void* workspace,
+                                  size_t workspace_bytes, b200asr_stream stream) {
+    B200_REQUIRE(a_hi && a_lo && a_sinv && b_hi && b_lo && b_sinv && C, "gemm_f16x3: null pointer");
+    B200_REQUIRE(M > 0 && N > 0 && Kp > 0 && (Kp % F_CK) == 0 && ldc >= N,
+                 "gemm_f16x3: bad sizes M=%d N=%d Kp=%d ldc=%d (Kp must be b200asr_f16x3_padded_k of K)", M, N, Kp, ldc);
+    B200_REQUIRE(aligned16(a_hi) && aligned16(a_lo) && aligned16(b_hi) && aligned16(b_lo),
+                 "gemm_f16x3: images must be 16-byte aligned");
+    B200_REQUIRE(!permute_rows || (M % 4) == 0, "gemm_f16x3: the row permutation needs M %% 4 == 0");
+    CUtensorMap mah, mal, mbh, mbl;
+    int rc;
+    if ((rc = make_map_f16(&mah, a_hi, M, Kp)) != B200_OK) return rc;
+    if ((rc = make_map_f16(&mal, a_lo, M, Kp)) != B200_OK) return rc;
+    if ((rc = make_map_f16(&mbh, b_hi, N, Kp)) != B200_OK) return rc;
+    if ((rc = make_map_f16(&mbl, b_lo, N, Kp)) != B200_OK) return rc;
+    F16Args g = {};
+    g.bias = bias; g.sa = a_sinv; g.sb = b_sinv; g.C = C;
+    g.M = M; g.N = N; g.ldc = ldc; g.accumulate = accumulate; g.perm = permute_rows;
+    g.KB = Kp / F_BK;
+    // same split rule (and so the same workspace bound, b200asr_gemm3x_workspace_bytes) as the 3xTF32 kernel, in k
+    int nsplit = pick_split(M, N, Kp / G_BK);
+    if (nsplit > 1 && (workspace == nullptr || workspace_bytes < (size_t)nsplit * M * N * sizeof(float))) nsplit = 1;
+    const int chunks = g.KB / F_CH;
+    g.kb_per_split = (chunks + nsplit - 1) / nsplit * F_CH;
+    nsplit = (g.KB + g.kb_per_split - 1) / g.kb_per_split;
+    g.partial = reinterpret_cast<float*>(workspace);
+    const size_t smem = (size_t)F_STAGES * F_STAGE + 256;
+    cudaStream_t st = (cudaStream_t)stream;
+    B200_CUDA(cudaFuncSetAttribute(gemm_f16x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dim3 grid((N + G_BN - 1) / G_BN, (M + G_BM - 1) / G_BM, nsplit);
+    gemm_f16x3_kernel<<<grid, G_THREADS, smem, st>>>(mah, mal, mbh, mbl, g);
+    B200_LAUNCH_CHECK("gemm_f16x3_kernel");
+    if (nsplit > 1) {
+        const long long total = (long long)M * N;
+        int blocks = (int)((total + 255) / 256);
+        if (blocks > 16 * sm_count()) blocks = 16 * sm_count();
+        gemm3x_reduce_kernel<<<blocks, 256, 0, st>>>(g.partial, nsplit, bias, C, M, N, ldc, accumulate, permute_rows);
+        B200_LAUNCH_CHECK("gemm3x_reduce_kernel");
+    }
+    return B200_OK;
+}

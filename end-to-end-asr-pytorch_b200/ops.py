@@ -39,7 +39,7 @@ def gate_perm(H, device):
 # ----------------------------------------------------------------------------------------------------------
 # Dense contractions of the step (K6 / K9 / K11 and their autograd backward).  fp32 parity (1e-4 on logits after 4
 # recurrent layers) rules out single-pass TF32/BF16, so every product is error-compensated "3xTF32" (fp32 class).
-# GEMM_MODE "umma" (default): this library's own wgmma kernel (csrc/gemm.cu) in its three operand forms -
+# GEMM_MODE "umma": this library's own wgmma kernel (csrc/gemm.cu) in its three operand forms -
 #   gemm_tn  x . W^T (+ bias)   forward;   gemm_nn  dY . W   input gradient (W in place);   gemm_nt  dY^T . X   weight
 #   gradient (contraction over the B*T rows, h_prev read shifted from the layer output, gate permutation in the epilogue).
 #   A is split into hi / lo in registers (wgmma with A from registers); B's raw fp32 tile is its TF32 hi operand and
@@ -50,7 +50,11 @@ def gate_perm(H, device):
 #   residual anyway, and gemm_nt's a is gathered into registers with transposed addressing, so those forms take none.
 # GEMM_MODE "tf32x3": the same arithmetic as three cuBLAS TF32 GEMMs on operands split by b200asr_split_tf32 (kept as a
 #   cross-check and for shapes whose row pitch is not a multiple of 4 floats); "fp32": cuBLAS SGEMM on the CUDA cores.
-GEMM_MODE = os.environ.get("B200ASR_GEMM", "umma")
+# GEMM_MODE "f16x3" (default): the four contractions of a BiLSTM layer (input projection, dX, dW_ih, dW_hh) run on
+#   scaled fp16 hi/lo images (f16_split / f16_split_t + gemm_f16x3: three fp16 tensor-core products, twice the 3xTF32
+#   rate); every other caller of the own GEMM runs "umma".
+GEMM_MODE = os.environ.get("B200ASR_GEMM", "f16x3")
+_OWN_GEMM = ("umma", "f16x3")
 
 
 def tf32_residual(w):
@@ -103,7 +107,7 @@ def gemm_tn(a, w, bias=None, out=None, accumulate=False, w_lo=None, a_lo=None):
 
 
 def _use_umma(K):
-    return GEMM_MODE == "umma" and K % 4 == 0
+    return GEMM_MODE in _OWN_GEMM and K % 4 == 0
 
 
 def gemm_tn_ld(a_base, lda, M, K, w, bias=None):
@@ -160,6 +164,58 @@ def gemm_nt(a, b, M, N, T, batches=1, lda=None, a_bstride=0, ldb=None, b_bstride
                                       T, batches, N, int(bool(accumulate)), int(bool(permute_rows)), L.ptr(ws),
                                       ws_bytes, L.stream()),
                 "gemm3x_nt")
+    return out
+
+
+def f16_split(x, rows, K, ld=None):
+    """K-major fp32 operand x[rows, K] (row pitch ld) -> f16x3 operand (img, sinv): img[0] / img[1] = the hi / lo fp16
+    images [rows, Kp] (K zero-padded to the 128-k scale chunk), sinv[Kp // 128, rows] = the inverse chunk scales."""
+    lib = L.load()
+    ld = K if ld is None else ld
+    Kp = lib.b200asr_f16x3_padded_k(K)
+    img = torch.empty((2, rows, Kp), device=x.device, dtype=torch.float16)
+    sinv = torch.empty((Kp // 128, rows), device=x.device, dtype=torch.float32)
+    with L.timed("f16_split", 4 * rows * K + 4 * rows * Kp):
+        L.check(lib.b200asr_f16x3_split_rows(L.ptr(x), ld, rows, K, L.ptr(img[0]), L.ptr(img[1]), L.ptr(sinv),
+                                             L.stream()), "f16x3_split_rows")
+    return img, sinv
+
+
+def f16_split_t(x, cols, T, batches=1, ld=None, bstride=0, shift=0):
+    """MN-major fp32 operand (element (b, t, c) at x[b*bstride + (t+shift)*ld + c], zero where t+shift is outside
+    [0, T); `x`'s data pointer is element (0, 0, 0)) -> f16x3 operand of its transpose: images [2, cols, Rp] over the
+    R = batches*T contraction rows, sinv[Rp // 128, cols]."""
+    lib = L.load()
+    ld = cols if ld is None else ld
+    Rp = lib.b200asr_f16x3_padded_k(batches * T)
+    img = torch.empty((2, cols, Rp), device=x.device, dtype=torch.float16)
+    sinv = torch.empty((Rp // 128, cols), device=x.device, dtype=torch.float32)
+    with L.timed("f16_split", 4 * batches * T * cols + 4 * cols * Rp):
+        L.check(lib.b200asr_f16x3_split_cols(L.ptr(x), ld, bstride, shift, T, batches, cols, L.ptr(img[0]),
+                                             L.ptr(img[1]), L.ptr(sinv), L.stream()), "f16x3_split_cols")
+    return img, sinv
+
+
+def gemm_f16x3(a, b, bias=None, out=None, accumulate=False, permute_rows=False, name="gemm_f16_tn"):
+    """out[M,N] (= or +=) A . B^T (+ bias[N]) for two f16x3 operands (f16_split / f16_split_t with the same Kp):
+    fp32-class products on the fp16 tensor cores (csrc/gemm.cu).  permute_rows writes row m to (m%4)*(M/4) + m/4."""
+    lib = L.load()
+    (aimg, asinv), (bimg, bsinv) = a, b
+    M, Kp = aimg.shape[1], aimg.shape[2]
+    N = bimg.shape[1]
+    assert bimg.shape[2] == Kp
+    if out is None:
+        out = torch.empty((M, N), device=aimg.device, dtype=torch.float32)
+        accumulate = False
+    assert out.dtype == torch.float32 and out.stride(1) == 1 and out.shape == (M, N)
+    ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
+    ws = torch.empty(max(ws_bytes, 16), device=aimg.device, dtype=torch.uint8)
+    bb = _f32c(bias) if bias is not None else None
+    with L.timed(name, 4 * Kp * (M + N) + 4 * M * N * (2 if accumulate else 1)):
+        L.check(lib.b200asr_gemm_f16x3(L.ptr(aimg[0]), L.ptr(aimg[1]), L.ptr(asinv), L.ptr(bimg[0]), L.ptr(bimg[1]),
+                                       L.ptr(bsinv), L.ptr(bb), L.ptr(out), M, N, Kp, out.stride(0),
+                                       int(bool(accumulate)), int(bool(permute_rows)), L.ptr(ws), ws_bytes,
+                                       L.stream()), "gemm_f16x3")
     return out
 
 
@@ -293,7 +349,11 @@ def mm1(a, b, out=None, bias=None, accumulate=False):
 
 
 def _gemm_ops():
-    return (Split, mm3) if GEMM_MODE in ("tf32x3", "umma") else (Plain, mm1)
+    return (Split, mm3) if GEMM_MODE in ("tf32x3",) + _OWN_GEMM else (Plain, mm1)
+
+
+def _use_f16x3(I, H):
+    return GEMM_MODE == "f16x3" and I % 4 == 0 and H % 4 == 0
 
 
 class BiLSTMFn(Function):
@@ -317,20 +377,24 @@ class BiLSTMFn(Function):
         H = params[1].shape[1]
         dev = x.device
         perm = gate_perm(H, dev)
+        f16 = _use_f16x3(I, H)
         umma = _use_umma(I)
         xs = None if umma else Op(x.view(B * T, I))
+        xi = f16_split(x.view(B * T, I), B * T, I) if f16 else None      # one image of x serves both directions
         gates = torch.empty((ndir, B, T, H, 4), device=dev, dtype=torch.float32)
         w_ih_p = []
         for d in range(ndir):
             w_ih, w_hh, b_ih, b_hh = params[4 * d:4 * d + 4]
             wp = w_ih.detach().index_select(0, perm)
             bp = (b_ih.detach() + b_hh.detach()).index_select(0, perm)
-            if umma:
+            if f16:
+                gemm_f16x3(xi, f16_split(wp, 4 * H, I), bias=bp, out=gates[d].view(B * T, 4 * H))
+            elif umma:
                 gemm_tn(x.view(B * T, I), wp, bias=bp, out=gates[d].view(B * T, 4 * H), w_lo=tf32_residual(wp))
             else:
                 mm(xs, Op(wp).t(), out=gates[d].view(B * T, 4 * H), bias=bp)
             w_ih_p.append(wp)
-        del xs
+        del xs, xi
         w_hh = torch.stack([_f32c(params[4 * d + 1].detach()) for d in range(ndir)]).contiguous()
         cst = torch.empty((ndir, B, T, H), device=dev, dtype=torch.float32)
         out = torch.empty((B, T, ndir * H), device=dev, dtype=torch.float32)
@@ -373,6 +437,26 @@ class BiLSTMFn(Function):
         need_dx = ctx.needs_input_grad[0]
         dx2 = torch.empty((B * T, I), device=dev, dtype=torch.float32) if need_dx else None
         grads = []
+        if _use_f16x3(I, H):
+            # dX = dG . W on the row images of dG and W^T; dW_ih = dG^T . X and dW_hh = dG^T . h_prev on transposed
+            # images (h_prev's written shifted by one step per utterance, zero at the sequence ends); rows written
+            # through the gate permutation by the epilogue.
+            xt = f16_split_t(x, I, B * T)
+            for d in range(ndir):
+                g2 = gates[d].view(B * T, 4 * H)
+                if need_dx:
+                    gemm_f16x3(f16_split(g2, B * T, 4 * H), f16_split(w_ih_p[d].t().contiguous(), I, 4 * H), out=dx2,
+                               accumulate=(d > 0))
+                gt = f16_split_t(g2, 4 * H, B * T)
+                dw_ih = gemm_f16x3(gt, xt, permute_rows=True, name="gemm_f16_nt")
+                hd = out[:, :, d * H:(d + 1) * H]
+                ht = f16_split_t(hd, H, T, batches=B, ld=ndir * H, bstride=T * ndir * H, shift=(-1 if d == 0 else 1))
+                dw_hh = gemm_f16x3(gt, ht, permute_rows=True, name="gemm_f16_nt")
+                del gt, ht
+                db = torch.empty((4 * H,), device=dev, dtype=torch.float32)
+                db.index_copy_(0, perm, g2.sum(0))
+                grads += [dw_ih, dw_hh, db, db.clone()]
+            return (dx2.view(B, T, I) if need_dx else None, None, *grads, *ctx.tail)
         if _use_umma(I) and H % 4 == 0:
             # own tensor-core kernels throughout: dX = dG . W as the tn form on W^T (one transposed copy and its residual
             # per layer and direction, so the kernel neither transposes nor splits the weight in every CTA),
@@ -749,7 +833,7 @@ def decoder_step(dw, x, h):
 
 
 def decoder_gemm_supported(I, H):
-    return GEMM_MODE == "umma" and (I + H) % 4 == 0 and (4 * H) % 4 == 0
+    return GEMM_MODE in _OWN_GEMM and (I + H) % 4 == 0 and (4 * H) % 4 == 0
 
 
 # ----------------------------------------------------------------------------------------------------------

@@ -281,6 +281,27 @@ B200ASR_API int b200asr_gemm3x_tn_pre2(const float* A, const float* A_lo, int ld
                            const float* bias, float* C, int M, int N, int K, int ldc, int accumulate, void* workspace,
                            size_t workspace_bytes, b200asr_stream stream);
 
+/* ---- f16x3: the BiLSTM layer contractions on scaled fp16 hi/lo images (GEMM_MODE "f16x3", the default) -------------
+ * An operand X[outer][k] (k = the contraction index) becomes two K-major fp16 images hi, lo [outer][Kp],
+ * Kp = b200asr_f16x3_padded_k(K) (K rounded up to the 128-k scale chunk, zero-filled), and inverse scales
+ * sinv[Kp / 128][outer]: per (outer index, 128-k chunk) a power of two s brings the chunk maximum to [2^13, 2^14),
+ * hi = f16(x s), lo = f16(x s - hi), sinv = 1 / s.  A chunk holding a NaN / Inf, or only zeros, gets s = 1.
+ *   _split_rows: K-major x (element (row, k) at x[row * ld + k]; K, ld multiples of 4, 16-byte aligned).
+ *   _split_cols: MN-major x, transposed: image row = column c, image column r = b T + t, element at
+ *     x[b * bstride + (t + shift) * ld + c], zero where t + shift is outside [0, T) (h_prev of a direction).
+ *   b200asr_gemm_f16x3:  C[M,N] (+)= sum_k A[m][k] B[n][k] (+ bias[N]) over the two operands' images (same Kp):
+ *     hi.hi + hi.lo + lo.hi per 16 k on the tensor cores, each 128-k chunk folded with its scales into an fp32
+ *     register sum; ldc, accumulate, permute_rows (row m -> (m % 4) * (M / 4) + m / 4) and the split-K workspace
+ *     (b200asr_gemm3x_workspace_bytes(M, N), may be NULL) as in b200asr_gemm3x_nt.                                 */
+B200ASR_API int b200asr_f16x3_padded_k(int K);
+B200ASR_API int b200asr_f16x3_split_rows(const float* x, long long ld, int rows, int K, void* hi, void* lo, float* sinv,
+                             b200asr_stream stream);
+B200ASR_API int b200asr_f16x3_split_cols(const float* x, long long ld, long long bstride, int shift, int T, int batches,
+                             int cols, void* hi, void* lo, float* sinv, b200asr_stream stream);
+B200ASR_API int b200asr_gemm_f16x3(const void* a_hi, const void* a_lo, const float* a_sinv, const void* b_hi, const void* b_lo,
+                       const float* b_sinv, const float* bias, float* C, int M, int N, int Kp, int ldc, int accumulate,
+                       int permute_rows, void* workspace, size_t workspace_bytes, b200asr_stream stream);
+
 /* ---- K6 helper: split fp32 into a TF32-representable high part and the fp32 residual ---------------------------
  * hi = x rounded to TF32, lo = x - hi; used to run the input-projection (src/module.py:131, inside nn.LSTM) and the
  * weight-gradient contractions as three error-compensated TF32 tensor-core GEMMs (3xTF32) at fp32-level accuracy.  */

@@ -1,13 +1,16 @@
-"""ms and TFLOP/s of the own wgmma 3xTF32 GEMM at the calls one cfg-B train step makes per BiLSTM layer and direction
+"""ms and TFLOP/s of the own wgmma GEMMs at the calls one cfg-B train step makes per BiLSTM layer and direction
 (input projection, input gradient and the transposed weight copy it needs, dW_ih, shifted dW_hh), with the share of
-the fp32-class ceiling: 3xTF32 runs three TF32 passes, so the ceiling is a third of the data-sheet dense TF32 rate (495 / 3 = 165 TFLOP/s on an H100 SXM at
-700 W).  Prints the card name and power limit of the run.  QUICK=1 times layer 3 only."""
+the fp32-class ceiling, for both paths: 3xTF32 runs three TF32 passes, so its ceiling is a third of the data-sheet dense
+TF32 rate (495 / 3 = 165 TFLOP/s on an H100 SXM at 700 W); f16x3 runs three fp16 products, a third of the data-sheet
+dense fp16 rate (989 / 3 = 330 TFLOP/s), and its operand preparation passes (f16_split, memory-bound) are timed as
+calls of their own.  Prints the card name and power limit of the run.  QUICK=1 times layer 3 only."""
 import importlib, os, subprocess, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 pkg = importlib.import_module("end-to-end-asr-pytorch_b200")
 ops = pkg.ops
 dev = "cuda"
 CEILING = 495.0 / 3        # TFLOP/s: H100 SXM data-sheet dense TF32 / 3 passes (a data-sheet figure, not measured)
+CEILING_F16 = 989.0 / 3    # TFLOP/s: H100 SXM data-sheet dense fp16 / 3 products (a data-sheet figure, not measured)
 H, B = 512, 64             # cfg B: hidden size per direction, utterances per step
 LAYERS = [(76672, 120), (76672, 1024), (38336, 2048), (19136, 2048)]      # (B*T rows, input width) per layer
 
@@ -30,7 +33,7 @@ q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,
 print("card: %s (name, power limit)" % (q or torch.cuda.get_device_name()))
 print("%-34s %6s %5s %5s %8s %8s %7s" % ("call", "M", "N", "K", "ms", "TFLOP/s", "ceiling"))
 layers = LAYERS[3:] if os.environ.get("QUICK") else LAYERS
-step_ms = step_tf = 0.0
+step_ms = step_tf = f16_ms = f16_prep_ms = 0.0
 for li, (rows, I) in ((i, l) for i, l in enumerate(LAYERS) if l in layers):
     T = rows // B
     x = torch.randn(rows, I, device=dev)
@@ -60,6 +63,37 @@ for li, (rows, I) in ((i, l) for i, l in enumerate(LAYERS) if l in layers):
         if "nn" not in name:                     # the step runs the tn form of dX; nn is listed for comparison
             step_ms += 2 * ms
             step_tf += 2 * 2.0 * M * N * K / 1e12
-    del x, w, g, h, wlo, wt, wtlo
+    # f16x3: the images one direction makes (x's and X^T's are made once per layer and shared by both directions:
+    # counted at half weight per direction)
+    xi, wi, gi = ops.f16_split(x, rows, I), ops.f16_split(w, 4 * H, I), ops.f16_split(g, rows, 4 * H)
+    wti, gt = ops.f16_split(wt, I, 4 * H), ops.f16_split_t(g, 4 * H, rows)
+    xt = ops.f16_split_t(x, I, rows)
+    ht = ops.f16_split_t(h, H, T, batches=B, ld=2 * H, bstride=T * 2 * H, shift=-1)
+    fcalls = [("L%d f16 split x (per layer)" % li, 0, 0, 0, 0.5, lambda: ops.f16_split(x, rows, I)),
+              ("L%d f16 split W" % li, 0, 0, 0, 1, lambda: ops.f16_split(w, 4 * H, I)),
+              ("L%d f16 input projection" % li, rows, 4 * H, I, 1, lambda: ops.gemm_f16x3(xi, wi))]
+    if li > 0:
+        fcalls += [("L%d f16 split dG" % li, 0, 0, 0, 1, lambda: ops.f16_split(g, rows, 4 * H)),
+                   ("L%d f16 split W^T (copy incl.)" % li, 0, 0, 0, 1, lambda: ops.f16_split(w.t().contiguous(), I, 4 * H)),
+                   ("L%d f16 dX" % li, rows, I, 4 * H, 1, lambda: ops.gemm_f16x3(gi, wti))]
+    fcalls += [("L%d f16 split dG^T" % li, 0, 0, 0, 1, lambda: ops.f16_split_t(g, 4 * H, rows)),
+               ("L%d f16 split X^T (per layer)" % li, 0, 0, 0, 0.5, lambda: ops.f16_split_t(x, I, rows)),
+               ("L%d f16 dW_ih" % li, 4 * H, I, rows, 1, lambda: ops.gemm_f16x3(gt, xt, permute_rows=True)),
+               ("L%d f16 split h_prev^T (shifted)" % li, 0, 0, 0, 1,
+                lambda: ops.f16_split_t(h, H, T, batches=B, ld=2 * H, bstride=T * 2 * H, shift=-1)),
+               ("L%d f16 dW_hh" % li, 4 * H, H, rows, 1, lambda: ops.gemm_f16x3(gt, ht, permute_rows=True))]
+    for name, M, N, K, wgt, fn in fcalls:
+        ms = timeit(fn)
+        if M == 0:
+            print("%-34s %26.3f" % (name, ms), flush=True)
+            f16_prep_ms += 2 * wgt * ms
+        else:
+            tf = 2.0 * M * N * K / ms / 1e9
+            print("%-34s %6d %5d %5d %8.3f %8.1f %6.1f%%" % (name, M, N, K, ms, tf, 100 * tf / CEILING_F16), flush=True)
+            f16_ms += 2 * ms
+    del x, w, g, h, wlo, wt, wtlo, xi, wi, gi, wti, gt, xt, ht
 print("sum over both directions: %.1f ms for %.2f TFLOP = %.1f TFLOP/s (%.1f%% of the %.0f TFLOP/s ceiling)"
       % (step_ms, step_tf, step_tf / step_ms * 1e3, 100 * step_tf / step_ms * 1e3 / CEILING, CEILING))
+print("f16x3, both directions: GEMMs %.1f ms = %.1f TFLOP/s (%.1f%% of the %.0f TFLOP/s ceiling), preparation passes "
+      "%.1f ms, together %.1f ms" % (f16_ms, step_tf / f16_ms * 1e3, 100 * step_tf / f16_ms * 1e3 / CEILING_F16,
+                                      CEILING_F16, f16_prep_ms, f16_ms + f16_prep_ms))
