@@ -753,11 +753,6 @@ int make_map_f16(CUtensorMap* map, const void* ptr, int rows, int Kp) {
 
 using namespace b200asr;
 
-extern "C" int b200asr_gemm3x_supported(int M, int N, int K) {
-    // TMA: 16-byte aligned row pitch; at least one full tile's worth of work is not required (tails are zero-filled)
-    return (M > 0 && N > 0 && K > 0 && (K % 4) == 0) ? 1 : 0;
-}
-
 extern "C" size_t b200asr_gemm3x_workspace_bytes(int M, int N) {
     if (M <= 0 || N <= 0) return 0;
     int s = max_split(M, N);                   // upper bound of what pick_split() may choose for any K
@@ -766,19 +761,14 @@ extern "C" size_t b200asr_gemm3x_workspace_bytes(int M, int N) {
     return s > 1 ? (size_t)s * M * N * sizeof(float) : 0;
 }
 
-extern "C" int b200asr_gemm3x_tn(const float* A, const float* B, const float* bias, float* C, int M, int N, int K,
-                                 int ldc, int accumulate, b200asr_stream stream) {
-    return b200asr_gemm3x_tn_ld(A, K, B, bias, C, M, N, K, ldc, accumulate, stream);
-}
-
-static int gemm3x_tn_impl(const float* A, int lda, const float* B, const float* bias, float* C, int M, int N, int K,
-                          int ldc, int accumulate, void* ws, size_t ws_bytes, b200asr_stream stream,
-                          const float* B_lo = nullptr, const float* A_lo = nullptr) {
+extern "C" int b200asr_gemm3x_tn(const float* A, int lda, const float* B, const float* B_lo, const float* bias, float* C,
+                                 int M, int N, int K, int ldc, int accumulate, void* workspace, size_t workspace_bytes,
+                                 b200asr_stream stream) {
     B200_REQUIRE(A && B && C, "gemm3x_tn: null pointer");
-    B200_REQUIRE(!A_lo || B_lo, "gemm3x_tn: a residual of A needs the residual of B as well");
     B200_REQUIRE(lda > 0 && (lda % 4) == 0, "gemm3x_tn: lda %d must be a positive multiple of 4", lda);
-    B200_REQUIRE(b200asr_gemm3x_supported(M, N, K), "gemm3x_tn: unsupported sizes M=%d N=%d K=%d (K %% 4 must be 0)", M,
-                 N, K);
+    // TMA: 16-byte aligned row pitch; at least one full tile's worth of work is not required (tails are zero-filled)
+    B200_REQUIRE(M > 0 && N > 0 && K > 0 && (K % 4) == 0,
+                 "gemm3x_tn: unsupported sizes M=%d N=%d K=%d (K %% 4 must be 0)", M, N, K);
     B200_REQUIRE(ldc >= N, "gemm3x_tn: ldc %d < N %d", ldc, N);
     B200_REQUIRE(aligned16(A) && aligned16(B), "gemm3x_tn: operands must be 16-byte aligned");
     CUtensorMap ma, mb;
@@ -794,26 +784,14 @@ static int gemm3x_tn_impl(const float* A, int lda, const float* B, const float* 
         CUtensorMap mlo;
         rc = make_map_k(&mlo, B_lo, N, K, K, G_BN);
         if (rc != B200_OK) return rc;
-        // A's residual is made in registers from the A fragment (A_lo holds the same values and is not read)
-        B200_REQUIRE(!A_lo || aligned16(A_lo), "gemm3x_tn: operands must be 16-byte aligned");
-        return launch<false, false, true>(ma, mb, g, ws, ws_bytes, (cudaStream_t)stream, &mlo);
+        return launch<false, false, true>(ma, mb, g, workspace, workspace_bytes, (cudaStream_t)stream, &mlo);
     }
-    return launch<false, false>(ma, mb, g, ws, ws_bytes, (cudaStream_t)stream);
+    return launch<false, false>(ma, mb, g, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
-extern "C" int b200asr_gemm3x_tn_ld(const float* A, int lda, const float* B, const float* bias, float* C, int M, int N,
-                                    int K, int ldc, int accumulate, b200asr_stream stream) {
-    return gemm3x_tn_impl(A, lda, B, bias, C, M, N, K, ldc, accumulate, nullptr, 0, stream);
-}
-
-extern "C" int b200asr_gemm3x_tn_ws(const float* A, int lda, const float* B, const float* bias, float* C, int M, int N,
-                                    int K, int ldc, int accumulate, void* workspace, size_t workspace_bytes,
-                                    b200asr_stream stream) {
-    return gemm3x_tn_impl(A, lda, B, bias, C, M, N, K, ldc, accumulate, workspace, workspace_bytes, stream);
-}
-
-static int gemm3x_nn_impl(const float* A, int lda, const float* B, int ldb, const float* bias, float* C, int M, int N,
-                          int K, int ldc, int accumulate, void* ws, size_t ws_bytes, b200asr_stream stream) {
+extern "C" int b200asr_gemm3x_nn(const float* A, int lda, const float* B, int ldb, const float* bias, float* C, int M,
+                                 int N, int K, int ldc, int accumulate, void* workspace, size_t workspace_bytes,
+                                 b200asr_stream stream) {
     B200_REQUIRE(A && B && C, "gemm3x_nn: null pointer");
     B200_REQUIRE(M > 0 && N > 0 && K > 0, "gemm3x_nn: bad sizes M=%d N=%d K=%d", M, N, K);
     B200_REQUIRE(lda >= K && (lda % 4) == 0 && ldb >= N && (ldb % 4) == 0 && ldc >= N,
@@ -827,18 +805,7 @@ static int gemm3x_nn_impl(const float* A, int lda, const float* B, int ldb, cons
     GemmArgs g = {};
     g.bias = bias; g.C = C; g.M = M; g.N = N; g.ldc = ldc; g.accumulate = accumulate;
     g.KB = (K + G_BK - 1) / G_BK; g.kbt = g.KB;
-    return launch<false, true>(ma, mb, g, ws, ws_bytes, (cudaStream_t)stream);
-}
-
-extern "C" int b200asr_gemm3x_nn(const float* A, int lda, const float* B, int ldb, const float* bias, float* C, int M,
-                                 int N, int K, int ldc, int accumulate, b200asr_stream stream) {
-    return gemm3x_nn_impl(A, lda, B, ldb, bias, C, M, N, K, ldc, accumulate, nullptr, 0, stream);
-}
-
-extern "C" int b200asr_gemm3x_nn_ws(const float* A, int lda, const float* B, int ldb, const float* bias, float* C, int M,
-                                    int N, int K, int ldc, int accumulate, void* workspace, size_t workspace_bytes,
-                                    b200asr_stream stream) {
-    return gemm3x_nn_impl(A, lda, B, ldb, bias, C, M, N, K, ldc, accumulate, workspace, workspace_bytes, stream);
+    return launch<false, true>(ma, mb, g, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int b200asr_gemm3x_nt(const float* A, long long lda, long long a_bstride, int a_shift, const float* B,
@@ -875,21 +842,6 @@ extern "C" int b200asr_tf32_residual(const float* x, float* lo, long long n, b20
     B200_LAUNCH_CHECK("tf32_residual_kernel");
     return B200_OK;
 }
-
-extern "C" int b200asr_gemm3x_tn_pre(const float* A, int lda, const float* B, const float* B_lo, const float* bias,
-                                     float* C, int M, int N, int K, int ldc, int accumulate, void* workspace,
-                                     size_t workspace_bytes, b200asr_stream stream) {
-    B200_REQUIRE(B_lo, "gemm3x_tn_pre: null residual");
-    return gemm3x_tn_impl(A, lda, B, bias, C, M, N, K, ldc, accumulate, workspace, workspace_bytes, stream, B_lo);
-}
-
-extern "C" int b200asr_gemm3x_tn_pre2(const float* A, const float* A_lo, int lda, const float* B, const float* B_lo,
-                                      const float* bias, float* C, int M, int N, int K, int ldc, int accumulate,
-                                      void* workspace, size_t workspace_bytes, b200asr_stream stream) {
-    B200_REQUIRE(A_lo && B_lo, "gemm3x_tn_pre2: null residual");
-    return gemm3x_tn_impl(A, lda, B, bias, C, M, N, K, ldc, accumulate, workspace, workspace_bytes, stream, B_lo, A_lo);
-}
-
 
 extern "C" int b200asr_f16x3_padded_k(int K) { return K > 0 ? (K + F_CK - 1) / F_CK * F_CK : 0; }
 

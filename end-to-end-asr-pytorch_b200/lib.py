@@ -66,23 +66,17 @@ SIGNATURES = {
     "b200asr_ce_fwd_bwd": (c_int, [_P, _P, c_longlong, c_longlong, c_int, _P, _P, _P, _P]),
     "b200asr_embedding_bwd_workspace_bytes": (c_size_t, [c_int, c_int]),
     "b200asr_embedding_bwd": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_size_t, _P]),
-    "b200asr_gemm3x_supported": (c_int, [c_int, c_int, c_int]),
-    "b200asr_gemm3x_tn": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
-    "b200asr_gemm3x_tn_ld": (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
-    "b200asr_gemm3x_nn": (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200asr_gemm3x_tn": (c_int, [_P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
+    "b200asr_gemm3x_nn": (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_gemm3x_workspace_bytes": (c_size_t, [c_int, c_int]),
-    "b200asr_gemm3x_tn_ws": (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
-    "b200asr_gemm3x_nn_ws": (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_gemm3x_nt": (c_int, [_P, c_longlong, c_longlong, c_int, _P, c_longlong, c_longlong, c_int, _P, c_int, c_int,
                                   c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_tf32_residual": (c_int, [_P, _P, c_longlong, _P]),
-    "b200asr_gemm3x_tn_pre": (c_int, [_P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_f16x3_padded_k": (c_int, [c_int]),
     "b200asr_f16x3_split_rows": (c_int, [_P, c_longlong, c_int, c_int, _P, _P, _P, _P]),
     "b200asr_f16x3_split_cols": (c_int, [_P, c_longlong, c_longlong, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
     "b200asr_gemm_f16x3": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_size_t,
                                    _P]),
-    "b200asr_gemm3x_tn_pre2": (c_int, [_P, _P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_split_tf32": (c_int, [_P, _P, _P, c_longlong, _P]),
     "b200asr_grad_norm_scratch_bytes": (c_size_t, []),
     "b200asr_grad_norm": (c_int, [_P, c_longlong, _P, _P, _P]),

@@ -3,7 +3,7 @@ n_layers, dropout), same parameter containers, state_dict keys and initialisatio
 
 LSTM (the lm_example configuration) runs on this library's kernels:
   - embedding: ATen row gather forward, ops.EmbeddingFn backward (b200asr_embedding_bwd, in place into the gradient);
-  - each layer: ops.bilstm(ndir=1), the persistent recurrence plus 3xTF32 input / weight-gradient GEMMs, over the padded
+  - each layer: ops.bilstm(ndir=1), the persistent recurrence plus f16x3 input / weight-gradient GEMMs, over the padded
     frames.  A row's outputs at t < len do not depend on later frames, so the packed result is the padded one with the
     output zeroed at t >= len; (h_n, c_n) are read from the output and the cell-state stash at t = len - 1.  Every
     padded target is ignored by the loss, so the gradient at padded frames is exactly zero and the backward is the

@@ -1,9 +1,11 @@
 """Encoder / attention building blocks with the reference's constructor signatures and state_dict keys
 (/root/reference/src/module.py), computing through the b200asr kernels.
 
-  RNNLayer               -> persistent BiLSTM kernels (ops.bilstm) + cuBLAS input/weight-grad GEMMs
+  RNNLayer               -> persistent BiLSTM kernels (ops.bilstm) + f16x3 input/weight-grad GEMMs (csrc/gemm.cu;
+                            the cuBLAS 3xTF32 composition when the input width is not a multiple of 4)
   LocationAwareAttention -> fused single-launch attention step (ops.loc_attention_step)
-  CNNExtractor / VGGExtractor / ScaleDotAttention -> library convolutions / GEMMs (cuDNN, cuBLAS); these are
+  CNNExtractor           -> its Conv1d(k 4, s 2) on the 3xTF32 GEMM kernel (ops.conv1d_k4s2p1)
+  VGGExtractor / ScaleDotAttention -> library convolutions / GEMMs (cuDNN, cuBLAS); these are
       plain dense contractions outside the four north-star kernels (SURVEY.md 8(f) rank 4).
 """
 import torch

@@ -38,8 +38,13 @@ def gate_perm(H, device):
 
 # ----------------------------------------------------------------------------------------------------------
 # Dense contractions of the step (K6 / K9 / K11 and their autograd backward).  fp32 parity (1e-4 on logits after 4
-# recurrent layers) rules out single-pass TF32/BF16, so every product is error-compensated "3xTF32" (fp32 class).
-# GEMM_MODE "umma": this library's own wgmma kernel (csrc/gemm.cu) in its three operand forms -
+# recurrent layers) rules out single-pass TF32/BF16, so every product is error-compensated (fp32 class).  Which
+# implementation runs follows from the shapes alone:
+# - The four contractions of a BiLSTM layer (input projection, dX, dW_ih, dW_hh) run on scaled fp16 hi/lo images
+#   (f16_split / f16_split_t + gemm_f16x3: three fp16 tensor-core products, twice the 3xTF32 rate) when the input width
+#   is a multiple of 4, else as three cuBLAS TF32 GEMMs on operands split by b200asr_split_tf32 (Split + mm3).
+# - Every other dense contraction (Conv1d prenet, Linear3xFn, CTC head, decoder step, tied LM projection) runs on this
+#   library's own 3xTF32 wgmma kernel (csrc/gemm.cu) in its three operand forms -
 #   gemm_tn  x . W^T (+ bias)   forward;   gemm_nn  dY . W   input gradient (W in place);   gemm_nt  dY^T . X   weight
 #   gradient (contraction over the B*T rows, h_prev read shifted from the layer output, gate permutation in the epilogue).
 #   A is split into hi / lo in registers (wgmma with A from registers); B's raw fp32 tile is its TF32 hi operand and
@@ -48,13 +53,7 @@ def gate_perm(H, device):
 #   The K-major w of gemm_tn may bring its residual pre-computed (tf32_residual: the weights, once per
 #   step); an MN-major B (w of gemm_nn, b of gemm_nt) passes through the kernel's transposing pass, which makes its
 #   residual anyway, and gemm_nt's a is gathered into registers with transposed addressing, so those forms take none.
-# GEMM_MODE "tf32x3": the same arithmetic as three cuBLAS TF32 GEMMs on operands split by b200asr_split_tf32 (kept as a
-#   cross-check and for shapes whose row pitch is not a multiple of 4 floats); "fp32": cuBLAS SGEMM on the CUDA cores.
-# GEMM_MODE "f16x3" (default): the four contractions of a BiLSTM layer (input projection, dX, dW_ih, dW_hh) run on
-#   scaled fp16 hi/lo images (f16_split / f16_split_t + gemm_f16x3: three fp16 tensor-core products, twice the 3xTF32
-#   rate); every other caller of the own GEMM runs "umma".
-GEMM_MODE = os.environ.get("B200ASR_GEMM", "f16x3")
-_OWN_GEMM = ("umma", "f16x3")
+#   Shapes the kernel does not take (a row pitch that is not a multiple of 4 floats) go through Split + mm3.
 
 
 def tf32_residual(w):
@@ -68,10 +67,9 @@ def tf32_residual(w):
     return lo
 
 
-def gemm_tn(a, w, bias=None, out=None, accumulate=False, w_lo=None, a_lo=None):
+def gemm_tn(a, w, bias=None, out=None, accumulate=False, w_lo=None):
     """out[M,N] (= or +=) a[M,K] @ w[N,K]^T (+ bias[N]) on the tensor cores at fp32-class accuracy (csrc/gemm.cu).
-    w_lo = tf32_residual(w) selects the pre-split form.  a_lo = tf32_residual(a) selects the pre2 entry point, which
-    computes the same products: the kernel makes A's residual in registers either way."""
+    w_lo = tf32_residual(w) selects the pre-split form."""
     lib = L.load()
     a, w = _f32c(a), _f32c(w)
     M, K = a.shape
@@ -81,33 +79,16 @@ def gemm_tn(a, w, bias=None, out=None, accumulate=False, w_lo=None, a_lo=None):
         accumulate = False
     assert out.stride(1) == 1 and out.shape == (M, N)
     b = _f32c(bias) if bias is not None else None
+    ws, ws_bytes = None, 0
+    # split-K over all SMs for a small tile grid: pre-split calls and skinny ones (the decoder's per-step products)
+    if w_lo is not None or M <= 256:
+        ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
+        ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
     # algorithmic bytes: both operands and the result once; flops 2*M*N*K (x3 tensor-core products)
     with L.timed("gemm3x_tn", 4 * (M * K + N * K + M * N * (2 if accumulate else 1))):
-        if w_lo is not None and a_lo is not None:
-            ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
-            ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
-            L.check(lib.b200asr_gemm3x_tn_pre2(L.ptr(a), L.ptr(a_lo), K, L.ptr(w), L.ptr(w_lo), L.ptr(b), L.ptr(out), M, N, K,
-                                               out.stride(0), int(bool(accumulate)), L.ptr(ws), ws_bytes, L.stream()),
-                    "gemm3x_tn_pre2")
-        elif w_lo is not None:
-            ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
-            ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
-            L.check(lib.b200asr_gemm3x_tn_pre(L.ptr(a), K, L.ptr(w), L.ptr(w_lo), L.ptr(b), L.ptr(out), M, N, K,
-                                              out.stride(0), int(bool(accumulate)), L.ptr(ws), ws_bytes, L.stream()),
-                    "gemm3x_tn_pre")
-        elif M <= 256:          # skinny (the decoder's per-step products): split-K over all SMs
-            ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
-            ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
-            L.check(lib.b200asr_gemm3x_tn_ws(L.ptr(a), K, L.ptr(w), L.ptr(b), L.ptr(out), M, N, K, out.stride(0),
-                                             int(bool(accumulate)), L.ptr(ws), ws_bytes, L.stream()), "gemm3x_tn_ws")
-        else:
-            L.check(lib.b200asr_gemm3x_tn(L.ptr(a), L.ptr(w), L.ptr(b), L.ptr(out), M, N, K, out.stride(0),
-                                          int(bool(accumulate)), L.stream()), "gemm3x_tn")
+        L.check(lib.b200asr_gemm3x_tn(L.ptr(a), K, L.ptr(w), L.ptr(w_lo), L.ptr(b), L.ptr(out), M, N, K, out.stride(0),
+                                      int(bool(accumulate)), L.ptr(ws), ws_bytes, L.stream()), "gemm3x_tn")
     return out
-
-
-def _use_umma(K):
-    return GEMM_MODE in _OWN_GEMM and K % 4 == 0
 
 
 def gemm_tn_ld(a_base, lda, M, K, w, bias=None):
@@ -118,8 +99,8 @@ def gemm_tn_ld(a_base, lda, M, K, w, bias=None):
     out = torch.empty((M, N), device=w.device, dtype=torch.float32)
     b = _f32c(bias) if bias is not None else None
     with L.timed("gemm3x_tn", 4 * (M * lda + N * K + M * N)):
-        L.check(lib.b200asr_gemm3x_tn_ld(L.ptr(a_base), lda, L.ptr(w), L.ptr(b), L.ptr(out), M, N, K, N, 0, L.stream()),
-                "gemm3x_tn_ld")
+        L.check(lib.b200asr_gemm3x_tn(L.ptr(a_base), lda, L.ptr(w), None, L.ptr(b), L.ptr(out), M, N, K, N, 0, None, 0,
+                                      L.stream()), "gemm3x_tn")
     return out
 
 
@@ -133,15 +114,13 @@ def gemm_nn(a, w, out=None, accumulate=False):
         out = torch.empty((M, N), device=a.device, dtype=torch.float32)
         accumulate = False
     assert out.stride(1) == 1 and out.shape == (M, N)
+    ws, ws_bytes = None, 0
+    if M <= 256:                        # skinny: split-K as in gemm_tn
+        ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
+        ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
     with L.timed("gemm3x_nn", 4 * (M * K + N * K + M * N * (2 if accumulate else 1))):
-        if M <= 256:
-            ws_bytes = lib.b200asr_gemm3x_workspace_bytes(M, N)
-            ws = torch.empty(max(ws_bytes, 16), device=a.device, dtype=torch.uint8)
-            L.check(lib.b200asr_gemm3x_nn_ws(L.ptr(a), K, L.ptr(w), N, None, L.ptr(out), M, N, K, out.stride(0),
-                                             int(bool(accumulate)), L.ptr(ws), ws_bytes, L.stream()), "gemm3x_nn_ws")
-        else:
-            L.check(lib.b200asr_gemm3x_nn(L.ptr(a), K, L.ptr(w), N, None, L.ptr(out), M, N, K, out.stride(0),
-                                          int(bool(accumulate)), L.stream()), "gemm3x_nn")
+        L.check(lib.b200asr_gemm3x_nn(L.ptr(a), K, L.ptr(w), N, None, L.ptr(out), M, N, K, out.stride(0),
+                                      int(bool(accumulate)), L.ptr(ws), ws_bytes, L.stream()), "gemm3x_nn")
     return out
 
 
@@ -271,8 +250,8 @@ class Conv1dK4S2Fn(Function):
 def conv1d_k4s2p1(x, conv):
     """[B,T,C] -> [B,T//2,O] through the tensor-core GEMM when available, else the library convolution."""
     C = x.shape[-1]
-    if (x.is_cuda and _use_umma(4 * C) and conv.kernel_size == (4,) and conv.stride == (2,) and conv.padding == (1,)
-            and x.shape[1] >= 2 and (2 * C) % 4 == 0):
+    if (x.is_cuda and conv.kernel_size == (4,) and conv.stride == (2,) and conv.padding == (1,) and x.shape[1] >= 2
+            and (2 * C) % 4 == 0):
         return Conv1dK4S2Fn.apply(x, conv.weight, conv.bias)
     return conv(x.transpose(1, 2)).transpose(1, 2)
 
@@ -321,47 +300,13 @@ def mm3(a, b, out=None, bias=None, accumulate=False):
     return out
 
 
-class Plain:
-    """Same interface as Split for the exact-fp32 SGEMM mode."""
-
-    def __init__(self, x):
-        self.x = _f32c(x)
-
-    def t(self):
-        o = object.__new__(Plain)
-        o.x = self.x.t()
-        return o
-
-    def view(self, *shape):
-        o = object.__new__(Plain)
-        o.x = self.x.view(*shape)
-        return o
-
-
-def mm1(a, b, out=None, bias=None, accumulate=False):
-    if out is None:
-        return torch.mm(a.x, b.x) if bias is None else torch.addmm(bias, a.x, b.x)
-    if accumulate:
-        return out.addmm_(a.x, b.x)
-    if bias is not None:
-        return torch.addmm(bias, a.x, b.x, out=out)
-    return torch.mm(a.x, b.x, out=out)
-
-
-def _gemm_ops():
-    return (Split, mm3) if GEMM_MODE in ("tf32x3",) + _OWN_GEMM else (Plain, mm1)
-
-
-def _use_f16x3(I, H):
-    return GEMM_MODE == "f16x3" and I % 4 == 0 and H % 4 == 0
-
-
 class BiLSTMFn(Function):
     """One (bi)directional LSTM layer over zero-padded frames, zero initial state (src/module.py:129-132).
 
     forward(x[B,T,I], ndir, w_ih_0, w_hh_0, b_ih_0, b_hh_0 [, w_ih_1, w_hh_1, b_ih_1, b_hh_1]) -> out[B,T,ndir*H]
-    The input projection and the weight-gradient contractions are tensor-core GEMMs (see GEMM_MODE); the recurrence
-    (forward and BPTT) is the persistent kernel pair b200asr_bilstm_fwd / b200asr_bilstm_bwd.
+    The input projection and the weight-gradient contractions are tensor-core GEMMs: f16x3 when I % 4 == 0, else the
+    cuBLAS 3xTF32 composition (Split + mm3); the recurrence (forward and BPTT) is the persistent kernel pair
+    b200asr_bilstm_fwd / b200asr_bilstm_bwd, which needs H % 16 == 0.
     """
 
     @staticmethod
@@ -371,16 +316,17 @@ class BiLSTMFn(Function):
         if params and isinstance(params[-1], CStateSink):
             sink, params = params[-1], params[:-1]
         assert len(params) == 4 * ndir
-        Op, mm = _gemm_ops()
         x = _f32c(x)
         B, T, I = x.shape
         H = params[1].shape[1]
         dev = x.device
+        ws_bytes = lib.b200asr_bilstm_workspace_bytes(B, T, H, ndir)
+        if ws_bytes == 0:
+            raise L.B200AsrError("bilstm: no feasible decomposition for B=%d H=%d (H must be a multiple of 16)" % (B, H))
         perm = gate_perm(H, dev)
-        f16 = _use_f16x3(I, H)
-        umma = _use_umma(I)
-        xs = None if umma else Op(x.view(B * T, I))
-        xi = f16_split(x.view(B * T, I), B * T, I) if f16 else None      # one image of x serves both directions
+        f16 = I % 4 == 0
+        # one operand of x serves both directions
+        xo = f16_split(x.view(B * T, I), B * T, I) if f16 else Split(x.view(B * T, I))
         gates = torch.empty((ndir, B, T, H, 4), device=dev, dtype=torch.float32)
         w_ih_p = []
         for d in range(ndir):
@@ -388,19 +334,14 @@ class BiLSTMFn(Function):
             wp = w_ih.detach().index_select(0, perm)
             bp = (b_ih.detach() + b_hh.detach()).index_select(0, perm)
             if f16:
-                gemm_f16x3(xi, f16_split(wp, 4 * H, I), bias=bp, out=gates[d].view(B * T, 4 * H))
-            elif umma:
-                gemm_tn(x.view(B * T, I), wp, bias=bp, out=gates[d].view(B * T, 4 * H), w_lo=tf32_residual(wp))
+                gemm_f16x3(xo, f16_split(wp, 4 * H, I), bias=bp, out=gates[d].view(B * T, 4 * H))
             else:
-                mm(xs, Op(wp).t(), out=gates[d].view(B * T, 4 * H), bias=bp)
+                mm3(xo, Split(wp).t(), out=gates[d].view(B * T, 4 * H), bias=bp)
             w_ih_p.append(wp)
-        del xs, xi
+        del xo
         w_hh = torch.stack([_f32c(params[4 * d + 1].detach()) for d in range(ndir)]).contiguous()
         cst = torch.empty((ndir, B, T, H), device=dev, dtype=torch.float32)
         out = torch.empty((B, T, ndir * H), device=dev, dtype=torch.float32)
-        ws_bytes = lib.b200asr_bilstm_workspace_bytes(B, T, H, ndir)
-        if ws_bytes == 0:
-            raise L.B200AsrError("bilstm: no feasible decomposition for B=%d H=%d (H must be a multiple of 16)" % (B, H))
         ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
         # algorithmic bytes (SURVEY.md 8(d)): per step and direction read Gx[t] (16BH) + write h,c (8BH); W_hh once
         with L.timed("bilstm_fwd", ndir * (24 * B * H * T + 16 * H * H)):
@@ -421,7 +362,6 @@ class BiLSTMFn(Function):
         if ctx.consumed:
             raise L.B200AsrError("BiLSTMFn.backward ran twice: the gate stash is overwritten in place")
         ctx.consumed = True
-        Op, mm = _gemm_ops()
         ndir = ctx.ndir
         B, T, I, H = ctx.dims
         x, gates, cst, out, w_hh = ctx.saved_tensors[:5]
@@ -436,65 +376,45 @@ class BiLSTMFn(Function):
         perm = gate_perm(H, dev)
         need_dx = ctx.needs_input_grad[0]
         dx2 = torch.empty((B * T, I), device=dev, dtype=torch.float32) if need_dx else None
-        grads = []
-        if _use_f16x3(I, H):
-            # dX = dG . W on the row images of dG and W^T; dW_ih = dG^T . X and dW_hh = dG^T . h_prev on transposed
-            # images (h_prev's written shifted by one step per utterance, zero at the sequence ends); rows written
-            # through the gate permutation by the epilogue.
+        f16 = I % 4 == 0
+        if f16:
             xt = f16_split_t(x, I, B * T)
-            for d in range(ndir):
-                g2 = gates[d].view(B * T, 4 * H)
+        else:
+            xs = Split(x.view(B * T, I))
+        grads = []
+        for d in range(ndir):
+            g2 = gates[d].view(B * T, 4 * H)      # d(loss)/d(pre-activation), unit-major columns
+            hd = out[:, :, d * H:(d + 1) * H]
+            if f16:
+                # dX = dG . W on the row images of dG and W^T; dW_ih = dG^T . X and dW_hh = dG^T . h_prev on transposed
+                # images (h_prev's written shifted by one step per utterance, zero at the sequence ends); rows written
+                # through the gate permutation by the epilogue.
                 if need_dx:
                     gemm_f16x3(f16_split(g2, B * T, 4 * H), f16_split(w_ih_p[d].t().contiguous(), I, 4 * H), out=dx2,
                                accumulate=(d > 0))
                 gt = f16_split_t(g2, 4 * H, B * T)
                 dw_ih = gemm_f16x3(gt, xt, permute_rows=True, name="gemm_f16_nt")
-                hd = out[:, :, d * H:(d + 1) * H]
                 ht = f16_split_t(hd, H, T, batches=B, ld=ndir * H, bstride=T * ndir * H, shift=(-1 if d == 0 else 1))
                 dw_hh = gemm_f16x3(gt, ht, permute_rows=True, name="gemm_f16_nt")
                 del gt, ht
-                db = torch.empty((4 * H,), device=dev, dtype=torch.float32)
-                db.index_copy_(0, perm, g2.sum(0))
-                grads += [dw_ih, dw_hh, db, db.clone()]
-            return (dx2.view(B, T, I) if need_dx else None, None, *grads, *ctx.tail)
-        if _use_umma(I) and H % 4 == 0:
-            # own tensor-core kernels throughout: dX = dG . W as the tn form on W^T (one transposed copy and its residual
-            # per layer and direction, so the kernel neither transposes nor splits the weight in every CTA),
-            # dW_ih = dG^T . X, dW_hh = dG^T . h_prev with h_prev read from the layer output shifted by one step (never
-            # materialised); rows written through the gate permutation by the epilogue.
-            for d in range(ndir):
-                g2 = gates[d].view(B * T, 4 * H)
+            else:
+                dG = Split(g2)
                 if need_dx:
-                    wt = w_ih_p[d].t().contiguous()
-                    gemm_tn(g2, wt, out=dx2, accumulate=(d > 0), w_lo=tf32_residual(wt))
-                dw_ih = gemm_nt(g2, x, 4 * H, I, B * T, permute_rows=True)
-                hd = out[:, :, d * H:(d + 1) * H]
-                dw_hh = gemm_nt(g2, hd, 4 * H, H, T, batches=B, a_bstride=T * 4 * H, ldb=ndir * H,
-                                b_bstride=T * ndir * H, b_shift=(-1 if d == 0 else 1), permute_rows=True)
-                db = torch.empty((4 * H,), device=dev, dtype=torch.float32)
-                db.index_copy_(0, perm, g2.sum(0))
-                grads += [dw_ih, dw_hh, db, db.clone()]
-            return (dx2.view(B, T, I) if need_dx else None, None, *grads, *ctx.tail)
-        xs = Op(x.view(B * T, I))
-        for d in range(ndir):
-            dG = Op(gates[d].view(B * T, 4 * H))  # d(loss)/d(pre-activation), unit-major columns
-            if need_dx:
-                mm(dG, Op(w_ih_p[d]), out=dx2, accumulate=(d > 0))
-            dw_ih = torch.empty((4 * H, I), device=dev, dtype=torch.float32)
-            dw_ih.index_copy_(0, perm, mm(dG.t(), xs))
+                    mm3(dG, Split(w_ih_p[d]), out=dx2, accumulate=(d > 0))
+                dw_ih = torch.empty((4 * H, I), device=dev, dtype=torch.float32)
+                dw_ih.index_copy_(0, perm, mm3(dG.t(), xs))
+                # h_{prev}: the hidden state of the previous step of this direction (zero at its first step)
+                hprev = torch.zeros((B, T, H), device=dev, dtype=torch.float32)
+                if T > 1:
+                    if d == 0:
+                        hprev[:, 1:] = hd[:, :-1]
+                    else:
+                        hprev[:, :-1] = hd[:, 1:]
+                dw_hh = torch.empty((4 * H, H), device=dev, dtype=torch.float32)
+                dw_hh.index_copy_(0, perm, mm3(dG.t(), Split(hprev.view(B * T, H))))
+                del dG, hprev
             db = torch.empty((4 * H,), device=dev, dtype=torch.float32)
-            db.index_copy_(0, perm, gates[d].view(B * T, 4 * H).sum(0))
-            # h_{prev}: the hidden state of the previous step of this direction (zero at its first step)
-            hprev = torch.zeros((B, T, H), device=dev, dtype=torch.float32)
-            hd = out[:, :, d * H:(d + 1) * H]
-            if T > 1:
-                if d == 0:
-                    hprev[:, 1:] = hd[:, :-1]
-                else:
-                    hprev[:, :-1] = hd[:, 1:]
-            dw_hh = torch.empty((4 * H, H), device=dev, dtype=torch.float32)
-            dw_hh.index_copy_(0, perm, mm(dG.t(), Op(hprev.view(B * T, H))))
-            del dG, hprev
+            db.index_copy_(0, perm, g2.sum(0))
             grads += [dw_ih, dw_hh, db, db.clone()]
         return (dx2.view(B, T, I) if need_dx else None, None, *grads, *ctx.tail)
 
@@ -833,7 +753,7 @@ def decoder_step(dw, x, h):
 
 
 def decoder_gemm_supported(I, H):
-    return GEMM_MODE in _OWN_GEMM and (I + H) % 4 == 0 and (4 * H) % 4 == 0
+    return (I + H) % 4 == 0
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -1069,19 +989,18 @@ def loc_attention_mem_step(mem, token, q, key, value, prev_att, enc_len, conv_w,
 # ----------------------------------------------------------------------------------------------------------
 class Linear3xFn(Function):
     """y = x W^T + b for the large dense layers of the step (CTC head, key projection, vocabulary projection) on
-    the tensor cores with the same error-compensated 3xTF32 scheme as the LSTM input projection (fp32-class)."""
+    the tensor cores with the error-compensated 3xTF32 scheme (fp32-class)."""
 
     @staticmethod
     def forward(ctx, x, weight, bias):
-        Op, mm = _gemm_ops()
         shp = x.shape
         x2 = _f32c(x).reshape(-1, shp[-1])
-        if _use_umma(x2.shape[1]):
+        if x2.shape[1] % 4 == 0:
             y = gemm_tn(x2, weight.detach(), bias=bias.detach() if bias is not None else None,
                         w_lo=tf32_residual(weight.detach()))
         else:
-            y = mm(Op(x2), Op(weight.detach()).t(), bias=bias.detach() if bias is not None else None,
-                   out=torch.empty((x2.shape[0], weight.shape[0]), device=x.device, dtype=torch.float32))
+            y = mm3(Split(x2), Split(weight.detach()).t(), bias=bias.detach() if bias is not None else None,
+                    out=torch.empty((x2.shape[0], weight.shape[0]), device=x.device, dtype=torch.float32))
         ctx.save_for_backward(x2, weight)
         ctx.shp = shp
         ctx.has_bias = bias is not None
@@ -1089,22 +1008,21 @@ class Linear3xFn(Function):
 
     @staticmethod
     def backward(ctx, gy):
-        Op, mm = _gemm_ops()
         x2, weight = ctx.saved_tensors
         gy2 = _f32c(gy).reshape(-1, weight.shape[0])
         dx = None
-        umma = _use_umma(weight.shape[0]) and _use_umma(weight.shape[1])
+        own = weight.shape[0] % 4 == 0 and weight.shape[1] % 4 == 0     # else (the CTC head at V = 31) Split + mm3
         if ctx.needs_input_grad[0]:
-            if umma:
+            if own:
                 dx = gemm_nn(gy2, weight.detach()).view(ctx.shp)
             else:
-                dx = mm(Op(gy2), Op(weight.detach())).view(ctx.shp)
+                dx = mm3(Split(gy2), Split(weight.detach())).view(ctx.shp)
         dw = None
         if ctx.needs_input_grad[1]:
-            if umma:
+            if own:
                 dw = gemm_nt(gy2, x2, weight.shape[0], weight.shape[1], gy2.shape[0])
             else:
-                dw = mm(Op(gy2).t(), Op(x2))
+                dw = mm3(Split(gy2).t(), Split(x2))
         db = gy.reshape(-1, weight.shape[0]).sum(0) if ctx.has_bias and ctx.needs_input_grad[2] else None
         return dx, dw, db
 
@@ -1183,7 +1101,7 @@ class TiedLinearFn(Function):
         shp = x.shape
         x2 = _f32c(x).reshape(-1, shp[-1])
         w = weight.detach()
-        if not (_use_umma(x2.shape[1]) and w.shape[0] % 4 == 0):
+        if not (x2.shape[1] % 4 == 0 and w.shape[0] % 4 == 0):
             raise L.B200AsrError("tied projection: E and V must be multiples of 4 for the tensor-core GEMM "
                                  "(E=%d V=%d)" % (x2.shape[1], w.shape[0]))
         y = gemm_tn(x2, w, w_lo=tf32_residual(w))

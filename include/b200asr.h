@@ -224,64 +224,49 @@ B200ASR_API int b200asr_adam_step(float* param, const float* grad, float* exp_av
                       float max_norm, b200asr_stream stream);
 
 /* ---- K6 / K9 / K11: dense  x . W^T (+ bias)  on the tensor cores at fp32-class accuracy ------------------------------
- * replaces the input projection inside nn.LSTM (src/module.py:112-113,131), the CTC head (src/asr.py:29,96) and the
- * proj_k / char_trans / pj Linear layers (src/asr.py:177,220,242-243; src/module.py:123,155) and their input gradients.
- *   C[M,N] (+)= A[M,K] . B[N,K]^T + bias[N]      A, B row-major with K contiguous (16-byte aligned, K % 4 == 0),
- *   C row-major with leading dimension ldc >= N; bias may be NULL; accumulate != 0 adds to the existing C.
+ * replaces the CTC head (src/asr.py:29,96), the proj_k / char_trans / pj Linear layers (src/asr.py:177,220,242-243;
+ * src/module.py:123,155), the decoder LSTM's projections (src/asr.py:214-221) and the Conv1d prenet (src/module.py:75-78),
+ * with their input and weight gradients.
  * wgmma tf32 with error compensation: A is split into hi / lo in registers, B's raw fp32 tile is its TF32 hi operand
- * (the tensor core truncates) and its residual tile is produced on the fly in shared memory; three products per K
- * block into one register accumulator. */
-B200ASR_API int b200asr_gemm3x_supported(int M, int N, int K);
-B200ASR_API int b200asr_gemm3x_tn(const float* A, const float* B, const float* bias, float* C, int M, int N, int K, int ldc,
-                      int accumulate, b200asr_stream stream);
-/* same with an explicit row pitch lda (floats, multiple of 4) of A.  lda < K is allowed: overlapping rows are the im2col
- * view of a strided 1-D convolution over a [time, channels] buffer (CNNExtractor, src/module.py:75-78: kernel 4, stride 2
- * -> K = 4*C, lda = 2*C), so the convolution runs in this kernel without materialising the windows. */
-B200ASR_API int b200asr_gemm3x_tn_ld(const float* A, int lda, const float* B, const float* bias, float* C, int M, int N, int K,
-                         int ldc, int accumulate, b200asr_stream stream);
-/* input gradient  dX = dY . W  (autograd backward of the Linear / LSTM input projection above):
+ * (the tensor core truncates) and B's residual tile is either made on the fly in shared memory or read pre-split; three
+ * products per K block into one register accumulator.
+ * Common arguments: C row-major with leading dimension ldc >= N; bias may be NULL; accumulate != 0 adds to the existing
+ * C.  workspace = NULL runs without split-K; otherwise it holds b200asr_gemm3x_workspace_bytes(M, N) bytes and small
+ * M x N tile grids with a long contraction (the decoder's per-step products, 64 rows) are cut along K over all SMs,
+ * partial tiles summed in a fixed order by a second launch (bias / accumulate applied there).
+ *
+ * tn:  C[M,N] (+)= A[M,K] . B[N,K]^T + bias[N]      A, B row-major with K contiguous (16-byte aligned, K % 4 == 0).
+ *   lda is A's row pitch (floats, multiple of 4).  lda < K is allowed: overlapping rows are the im2col view of a strided
+ *   1-D convolution over a [time, channels] buffer (CNNExtractor, src/module.py:75-78: kernel 4, stride 2 -> K = 4*C,
+ *   lda = 2*C), so the convolution runs in this kernel without materialising the windows.
+ *   B_lo = B - trunc_tf32(B) (b200asr_tf32_residual; same shape as B, dense rows of K floats) is the weight matrix'
+ *   residual computed once per step instead of once per tile by every CTA: its tile arrives by TMA like B's and no
+ *   shared-memory split pass runs.  B_lo = NULL: the kernel makes B's residual itself; the result is the same. */
+B200ASR_API int b200asr_gemm3x_tn(const float* A, int lda, const float* B, const float* B_lo, const float* bias, float* C,
+                      int M, int N, int K, int ldc, int accumulate, void* workspace, size_t workspace_bytes,
+                      b200asr_stream stream);
+/* nn: input gradient  dX = dY . W  (autograd backward of the layers above):
  *   C[M,N] (+)= A[M,K] . B[K,N] + bias[N]       A row-major with K contiguous (pitch lda), B row-major with N contiguous
- * (pitch ldb): the weight matrix is read in place as an MN-major tensor-core operand - no transposed copy. */
+ * (pitch ldb): the weight matrix is read in place as an MN-major tensor-core operand - no transposed copy; its residual
+ * is made in the kernel's transposing pass. */
 B200ASR_API int b200asr_gemm3x_nn(const float* A, int lda, const float* B, int ldb, const float* bias, float* C, int M, int N,
-                      int K, int ldc, int accumulate, b200asr_stream stream);
+                      int K, int ldc, int accumulate, void* workspace, size_t workspace_bytes, b200asr_stream stream);
 /* weight gradient  dW = dY^T . X  (autograd backward of the same layers; contraction over the batch*time rows):
  *   C[m,n] (+)= sum_{b < batches} sum_{t < T}  A[b][t + a_shift][m] * B[b][t + b_shift][n]
  * element (b, t, c) of an operand lives at ptr[b * bstride + t * ld + c] (both operands MN-major); rows outside [0, T)
  * read as zero, so  b_shift = -1 / +1  contracts dG[t] with the hidden state of the PREVIOUS step of the forward /
  * reverse direction (dW_hh of nn.LSTM) straight from the layer output.  permute_rows != 0 writes row m of the result
  * to row (m % 4) * (M / 4) + m / 4: from the kernels' unit-major gate order back to PyTorch's gate-major rows.
- * Small M x N with a long contraction is cut into split-K slices over all SMs (partials in `workspace`, summed in a
- * fixed order by a second launch); workspace may be NULL (no split).                                              */
+ * workspace as above.                                                                                               */
 B200ASR_API size_t b200asr_gemm3x_workspace_bytes(int M, int N);
-/* the tn / nn forms with a split-K workspace (b200asr_gemm3x_workspace_bytes(M, N)): skinny products - the decoder's
- * per-step  [B, in] . W^T  with B = 64 rows (src/asr.py:214-221) - are cut along K over all SMs, partial tiles summed in
- * a fixed order by a second launch (bias / accumulate applied there).                                              */
-B200ASR_API int b200asr_gemm3x_tn_ws(const float* A, int lda, const float* B, const float* bias, float* C, int M, int N, int K,
-                         int ldc, int accumulate, void* workspace, size_t workspace_bytes, b200asr_stream stream);
-B200ASR_API int b200asr_gemm3x_nn_ws(const float* A, int lda, const float* B, int ldb, const float* bias, float* C, int M,
-                         int N, int K, int ldc, int accumulate, void* workspace, size_t workspace_bytes,
-                         b200asr_stream stream);
 B200ASR_API int b200asr_gemm3x_nt(const float* A, long long lda, long long a_bstride, int a_shift, const float* B,
                       long long ldb, long long b_bstride, int b_shift, float* C, int M, int N, int T, int batches,
                       int ldc, int accumulate, int permute_rows, void* workspace, size_t workspace_bytes,
                       b200asr_stream stream);
-
-/* the tn form with PRE-SPLIT operands: B_lo = B - trunc_tf32(B) (b200asr_tf32_residual; same shape and pitch as B) is
- * the weight matrix' residual, computed once per step instead of once per tile by every CTA: its tile arrives by TMA
- * like B's and no shared-memory split pass runs.  _pre2 takes A_lo = A - trunc_tf32(A) (shape and pitch of A) as
- * well; the kernel makes the same values in registers, so it computes exactly what _pre computes.  Same residuals and
- * the same 12 products per K block as the other entry points.  workspace may be NULL.  Only a K-major B can bring a
- * residual: the MN-major B of the nn and nt forms goes through the kernel's transposing pass, which makes its
- * residual in the same sweep.                                                                                     */
+/* B_lo of the tn form: lo[i] = x[i] - trunc_tf32(x[i]) over n floats. */
 B200ASR_API int b200asr_tf32_residual(const float* x, float* lo, long long n, b200asr_stream stream);
-B200ASR_API int b200asr_gemm3x_tn_pre(const float* A, int lda, const float* B, const float* B_lo, const float* bias, float* C,
-                          int M, int N, int K, int ldc, int accumulate, void* workspace, size_t workspace_bytes,
-                          b200asr_stream stream);
-B200ASR_API int b200asr_gemm3x_tn_pre2(const float* A, const float* A_lo, int lda, const float* B, const float* B_lo,
-                           const float* bias, float* C, int M, int N, int K, int ldc, int accumulate, void* workspace,
-                           size_t workspace_bytes, b200asr_stream stream);
 
-/* ---- f16x3: the BiLSTM layer contractions on scaled fp16 hi/lo images (GEMM_MODE "f16x3", the default) -------------
+/* ---- f16x3: the BiLSTM layer contractions on scaled fp16 hi/lo images (input width a multiple of 4) ----------------
  * An operand X[outer][k] (k = the contraction index) becomes two K-major fp16 images hi, lo [outer][Kp],
  * Kp = b200asr_f16x3_padded_k(K) (K rounded up to the 128-k scale chunk, zero-filled), and inverse scales
  * sinv[Kp / 128][outer]: per (outer index, 128-k chunk) a power of two s brings the chunk maximum to [2^13, 2^14),

@@ -632,7 +632,7 @@ def test_ctc_prefix_score_vs_reference_scorer(pkg):
 
 @pytest.mark.parametrize("M,N,K,acc", [(3000, 2048, 1024, False), (300, 31, 120, False), (129, 257, 64, True),
                                       (1000, 5000, 2048, False), (77, 300, 2048, True), (5, 8, 4, False)])
-def test_gemm3x_umma_is_fp32_class(pkg, M, N, K, acc):
+def test_gemm3x_tn_is_fp32_class(pkg, M, N, K, acc):
     """csrc/gemm.cu (wgmma tf32, raw tiles as hi + on-the-fly residual tiles, register accumulator) must be as
     accurate as an fp32 SGEMM against an fp64 product - incl. M / N / K tails, bias, accumulate and ldc > N."""
     torch.manual_seed(M + N)
@@ -656,11 +656,6 @@ def test_gemm3x_umma_is_fp32_class(pkg, M, N, K, acc):
     pkg.ops.gemm_tn(a, b, bias=bias, out=out, accumulate=acc, w_lo=blo)
     e3 = scaled_err(out.cpu().numpy(), ref.cpu().numpy())
     assert e3 < 3e-6 and e3 < 20 * max(e1, 1e-7), (e3, e1)
-    # both operands pre-split: no in-kernel split pass at all
-    out.copy_(c0)
-    pkg.ops.gemm_tn(a, b, bias=bias, out=out, accumulate=acc, w_lo=blo, a_lo=pkg.ops.tf32_residual(a))
-    e3 = scaled_err(out.cpu().numpy(), ref.cpu().numpy())
-    assert e3 < 3e-6 and e3 < 20 * max(e1, 1e-7), (e3, e1)
     if acc:
         assert torch.equal(buf[:, N:], buf[:, N:])                              # padding columns untouched (no NaN)
 
@@ -676,10 +671,25 @@ def test_tf32_residual_pass(pkg, n):
         assert float(lo.abs().max()) <= float(v.abs().max()) * 2.0 ** -10
 
 
+def _kernel_names(pkg, fn):
+    """Run fn() with the kernel timer on: the names of the timed launches it made."""
+    timer = pkg.lib.TIMER
+    timer.reset()
+    timer.enabled = True
+    try:
+        fn()
+    finally:
+        timer.enabled = False
+    names = {r[0] for r in timer.records}
+    timer.reset()
+    return names
+
+
 @pytest.mark.parametrize("B,T,C,O", [(3, 41, 120, 640), (2, 10, 640, 640)])
-def test_conv1d_k4s2_through_the_gemm_kernel(pkg, B, T, C, O):
-    """CNNExtractor's Conv1d(k=4, s=2, p=1) as one wgmma GEMM over the in-place im2col view (overlapping rows,
-    lda = 2C < K = 4C) against the library convolution in fp64: output, input gradient, weight / bias gradients."""
+def test_conv1d_k4s2_selects_the_gemm_kernel(pkg, B, T, C, O):
+    """CNNExtractor's Conv1d(k=4, s=2, p=1) runs as one wgmma GEMM over the in-place im2col view (overlapping rows,
+    lda = 2C < K = 4C), checked against the library convolution in fp64: output, input gradient, weight / bias
+    gradients; its forward and both gradients go through the tn / nn / nt forms of csrc/gemm.cu."""
     torch.manual_seed(C + T)
     conv = torch.nn.Conv1d(C, O, 4, stride=2, padding=1)
     x = torch.randn(B, T, C)
@@ -691,13 +701,14 @@ def test_conv1d_k4s2_through_the_gemm_kernel(pkg, B, T, C, O):
     cd = torch.nn.Conv1d(C, O, 4, stride=2, padding=1).to(DEV)
     cd.load_state_dict(conv.state_dict())
     xd = x.to(DEV).requires_grad_(True)
-    mode, pkg.ops.GEMM_MODE = pkg.ops.GEMM_MODE, "umma"
-    try:
+
+    def step():
         y = pkg.ops.conv1d_k4s2p1(xd, cd)
         assert y.shape == ref.shape and scaled_err(y.detach().cpu().numpy(), ref.detach().numpy()) < 1e-5
         y.backward(gy.to(DEV))
-    finally:
-        pkg.ops.GEMM_MODE = mode
+
+    names = _kernel_names(pkg, step)
+    assert {"gemm3x_tn", "gemm3x_nn", "gemm3x_nt"} <= names, names
     assert scaled_err(xd.grad.cpu().numpy(), xr.grad.numpy()) < 1e-5
     wref = torch.autograd.grad(torch.nn.functional.conv1d(x.double().transpose(1, 2), conv.weight.double(),
                                                           conv.bias.double(), stride=2, padding=1).transpose(1, 2),
@@ -706,37 +717,39 @@ def test_conv1d_k4s2_through_the_gemm_kernel(pkg, B, T, C, O):
     assert scaled_err(cd.bias.grad.cpu().numpy(), wref[1].numpy()) < 1e-5
 
 
-def test_bilstm_and_linear_with_the_library_gemm_mode(pkg):
-    """GEMM_MODE 'tf32x3' (three cuBLAS TF32 GEMMs on b200asr_split_tf32 operands) stays a supported cross-check."""
-    mode, pkg.ops.GEMM_MODE = pkg.ops.GEMM_MODE, "tf32x3"
-    try:
-        _check_bilstm(pkg, 8, 13, 40, 320, True)
-        _check_bilstm(pkg, 64, 10, 120, 512, True)
-    finally:
-        pkg.ops.GEMM_MODE = mode
+def test_bilstm_gemm_path_follows_the_input_width(pkg):
+    """The BiLSTM layer's GEMMs follow the input width alone: I % 4 != 0 runs three cuBLAS TF32 GEMMs on
+    b200asr_split_tf32 operands (Split + mm3), I % 4 == 0 the f16x3 products and never the 3xTF32 kernel."""
+    for B, T, I, H in [(8, 13, 42, 320), (64, 10, 122, 512)]:
+        names = _kernel_names(pkg, lambda: _check_bilstm(pkg, B, T, I, H, True))
+        assert "split_tf32" in names and "f16_split" not in names, names
+    for B, T, I, H in [(8, 13, 40, 320), (64, 10, 120, 512)]:
+        names = _kernel_names(pkg, lambda: _check_bilstm(pkg, B, T, I, H, True))
+        assert "f16_split" in names and not any(n.startswith("gemm3x_") for n in names), names
 
 
-def test_linear_and_lstm_projection_through_the_gemm_kernel(pkg):
-    """GEMM_MODE 'umma': Linear3xFn and the BiLSTM input projection / input gradient through csrc/gemm.cu."""
-    mode, pkg.ops.GEMM_MODE = pkg.ops.GEMM_MODE, "umma"
-    try:
-        _check_bilstm(pkg, 8, 13, 40, 320, True)
-        torch.manual_seed(3)
-        lin = torch.nn.Linear(256, 1000)
-        x = torch.randn(4, 70, 256)
-        xr = x.double().requires_grad_(True)
-        ref = torch.nn.functional.linear(xr, lin.weight.detach().double(), lin.bias.detach().double())
-        g = torch.randn(4, 70, 1000)
-        ref.backward(g.double())
-        lin_d = torch.nn.Linear(256, 1000).to(DEV)
-        lin_d.load_state_dict(lin.state_dict())
-        xd = x.to(DEV).requires_grad_(True)
+def test_linear3x_fn_selects_the_gemm_kernel(pkg):
+    """Linear3xFn forward and input gradient against fp64; forward and both gradients go through the tn / nn / nt forms
+    of csrc/gemm.cu."""
+    torch.manual_seed(3)
+    lin = torch.nn.Linear(256, 1000)
+    x = torch.randn(4, 70, 256)
+    xr = x.double().requires_grad_(True)
+    ref = torch.nn.functional.linear(xr, lin.weight.detach().double(), lin.bias.detach().double())
+    g = torch.randn(4, 70, 1000)
+    ref.backward(g.double())
+    lin_d = torch.nn.Linear(256, 1000).to(DEV)
+    lin_d.load_state_dict(lin.state_dict())
+    xd = x.to(DEV).requires_grad_(True)
+
+    def step():
         y = pkg.ops.Linear3xFn.apply(xd, lin_d.weight, lin_d.bias)
         assert scaled_err(y.detach().cpu().numpy(), ref.detach().numpy()) < 1e-5
         y.backward(g.to(DEV))
-        assert scaled_err(xd.grad.cpu().numpy(), xr.grad.numpy()) < 1e-5
-    finally:
-        pkg.ops.GEMM_MODE = mode
+
+    names = _kernel_names(pkg, step)
+    assert {"gemm3x_tn", "gemm3x_nn", "gemm3x_nt"} <= names, names
+    assert scaled_err(xd.grad.cpu().numpy(), xr.grad.numpy()) < 1e-5
 
 
 @pytest.mark.parametrize("M,N,K,acc", [(3000, 2048, 1024, False), (300, 120, 2048, False), (129, 260, 64, True),

@@ -3,7 +3,9 @@
 the fp32-class ceiling, for both paths: 3xTF32 runs three TF32 passes, so its ceiling is a third of the data-sheet dense
 TF32 rate (495 / 3 = 165 TFLOP/s on an H100 SXM at 700 W); f16x3 runs three fp16 products, a third of the data-sheet
 dense fp16 rate (989 / 3 = 330 TFLOP/s), and its operand preparation passes (f16_split, memory-bound) are timed as
-calls of their own.  Prints the card name and power limit of the run.  QUICK=1 times layer 3 only."""
+calls of their own.  The step runs these contractions on f16x3; the 3xTF32 rows (through ops.gemm_tn / gemm_nn /
+gemm_nt) are a comparison of the two kernels at the same shapes, not calls the step makes.  Prints the card name and
+power limit of the run.  QUICK=1 times layer 3 only."""
 import importlib, os, subprocess, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 pkg = importlib.import_module("end-to-end-asr-pytorch_b200")
