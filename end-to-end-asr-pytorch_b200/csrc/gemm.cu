@@ -633,6 +633,94 @@ __global__ void __launch_bounds__(256) f16_split_cols_kernel(const float* __rest
     }
 }
 
+// The gate gradient dG of every direction, g[d][r][c] (R = B T rows, cols = 4 H unit-major columns), read once for the
+// three things the layer backward needs from it: the transposed images of each direction (dW_ih, dW_hh; as
+// f16_split_cols_kernel), optionally the row images of all directions side by side (dX; as f16_split_rows_kernel, with
+// direction d in image columns [d Kp, (d + 1) Kp) and scale chunks [d Kp / F_CK, (d + 1) Kp / F_CK)), and the column
+// sums of each 128-row tile (the bias gradient, reduced afterwards in a fixed order: no atomics).  One CTA per (128
+// rows, 128 columns, direction) staged in shared memory: its 128 columns of a row are one row-image chunk and its 128
+// rows of a column one transposed-image chunk, so every scale and image element comes out of the same values through
+// the same f16_scale_exp / f16_split2 as in the single-image passes, bit for bit.
+constexpr int DG_PITCH = F_CK + 4;        // staged row pitch (floats): float4 stores, conflict-free float4 column reads
+constexpr int DG_SMEM = F_CK * DG_PITCH * 4;
+
+__global__ void __launch_bounds__(256, 3) f16_split_dg_kernel(const float* __restrict__ g, int R, int cols, int Kp,
+                                                              int Rp, __half* __restrict__ t_hi,
+                                                              __half* __restrict__ t_lo, float* __restrict__ t_sinv,
+                                                              __half* __restrict__ r_hi, __half* __restrict__ r_lo,
+                                                              float* __restrict__ r_sinv, float* __restrict__ colsum) {
+    extern __shared__ float4 dg_smem[];
+    float* tile = reinterpret_cast<float*>(dg_smem);
+    const int r0 = blockIdx.x * F_CK, c0 = blockIdx.y * F_CK, d = blockIdx.z, ndir = gridDim.z;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const float* gd = g + (size_t)d * R * cols;
+    // rows warp + 8 i, 4 columns per lane: stage them, and write their row images (8 rows per batch of loads in flight)
+    const int c = c0 + 4 * lane;
+    const size_t ldr = (size_t)ndir * Kp;
+#pragma unroll
+    for (int i0 = 0; i0 < F_CK / 8; i0 += 8) {
+        float4 v[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const int r = r0 + warp + 8 * (i0 + i);
+            v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (r < R && c < cols) v[i] = *reinterpret_cast<const float4*>(gd + (size_t)r * cols + c);   // cols % 4 == 0
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const int rr = warp + 8 * (i0 + i), r = r0 + rr;
+            *reinterpret_cast<float4*>(tile + rr * DG_PITCH + 4 * lane) = v[i];
+            if (r_hi != nullptr && r < R) {
+                const uint32_t a = __reduce_max_sync(0xffffffffu, max(max(abs_bits(v[i].x), abs_bits(v[i].y)),
+                                                                      max(abs_bits(v[i].z), abs_bits(v[i].w))));
+                const int e = f16_scale_exp(a);
+                const float s = pow2f(e);
+                __half2 h[2], l[2];
+                f16_split2(v[i].x, v[i].y, s, h[0], l[0]);
+                f16_split2(v[i].z, v[i].w, s, h[1], l[1]);
+                const size_t o = (size_t)r * ldr + (size_t)d * Kp + c;
+                *reinterpret_cast<uint2*>(r_hi + o) = *reinterpret_cast<const uint2*>(h);
+                *reinterpret_cast<uint2*>(r_lo + o) = *reinterpret_cast<const uint2*>(l);
+                if (lane == 0) r_sinv[(size_t)(d * (Kp / F_CK) + blockIdx.y) * R + r] = pow2f(-e);
+            }
+        }
+    }
+    __syncthreads();
+    // warp w: column groups 4 (w + 8 j) .. + 3; lane holds rows lane + 32 i of the group's 4 columns
+    const size_t t_img = (size_t)d * cols * Rp, t_sc = (size_t)d * (Rp / F_CK) * cols;
+    for (int j = 0; j < F_CK / 32; ++j) {
+        const int cc = 4 * (warp + 8 * j), col0 = c0 + cc;
+        if (col0 >= cols) break;
+        float4 u[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) u[i] = *reinterpret_cast<const float4*>(tile + (lane + 32 * i) * DG_PITCH + cc);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const float x0 = (&u[0].x)[q], x1 = (&u[1].x)[q], x2 = (&u[2].x)[q], x3 = (&u[3].x)[q];
+            const int col = col0 + q;
+            const uint32_t a = __reduce_max_sync(0xffffffffu, max(max(abs_bits(x0), abs_bits(x1)),
+                                                                  max(abs_bits(x2), abs_bits(x3))));
+            const int e = f16_scale_exp(a);
+            const float s = pow2f(e);
+            __half2 h01, l01, h23, l23;                 // (rows lane, lane + 32), (lane + 64, lane + 96)
+            f16_split2(x0, x1, s, h01, l01);
+            f16_split2(x2, x3, s, h23, l23);
+            const size_t o = t_img + (size_t)col * Rp + r0 + lane;
+            t_hi[o] = __low2half(h01); t_hi[o + 32] = __high2half(h01);
+            t_hi[o + 64] = __low2half(h23); t_hi[o + 96] = __high2half(h23);
+            t_lo[o] = __low2half(l01); t_lo[o + 32] = __high2half(l01);
+            t_lo[o + 64] = __low2half(l23); t_lo[o + 96] = __high2half(l23);
+            float sum = (x0 + x1) + (x2 + x3);
+#pragma unroll
+            for (int m = 16; m > 0; m >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, m);
+            if (lane == 0) {
+                t_sinv[t_sc + (size_t)blockIdx.x * cols + col] = pow2f(-e);
+                colsum[(size_t)blockIdx.x * ndir * cols + (size_t)d * cols + col] = sum;
+            }
+        }
+    }
+}
+
 // One accumulation chunk (F_CH K blocks, starting at block i0 of the slice) into d (overwritten): block j + 1 is issued
 // before block j is waited for, the wait that retires a block releases its stage, the chunk ends in the only drain.
 __device__ __forceinline__ void f16_chunk(float (&d)[64], int i0, const uint8_t* smem, uint64_t* full, uint64_t* empty,
@@ -871,6 +959,26 @@ extern "C" int b200asr_f16x3_split_cols(const float* x, long long ld, long long 
     f16_split_cols_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ld, bstride, shift, T, R, cols, Rp, (__half*)hi,
                                                                   (__half*)lo, sinv);
     B200_LAUNCH_CHECK("f16_split_cols_kernel");
+    return B200_OK;
+}
+
+extern "C" int b200asr_f16x3_split_dg(const float* g, int ndir, int rows, int cols, void* t_hi, void* t_lo,
+                                      float* t_sinv, void* r_hi, void* r_lo, float* r_sinv, float* colsum,
+                                      b200asr_stream stream) {
+    B200_REQUIRE(g && t_hi && t_lo && t_sinv && colsum, "f16x3_split_dg: null pointer");
+    B200_REQUIRE((r_hi && r_lo && r_sinv) || (!r_hi && !r_lo && !r_sinv),
+                 "f16x3_split_dg: the row images need all of hi, lo and sinv (or none of them)");
+    B200_REQUIRE((ndir == 1 || ndir == 2) && rows > 0 && cols > 0 && (cols % 4) == 0 && aligned16(g),
+                 "f16x3_split_dg: needs 1 or 2 directions, cols %% 4 == 0, 16-byte alignment (ndir %d rows %d cols %d)",
+                 ndir, rows, cols);
+    B200_REQUIRE(rows < (1 << 30) && cols < (1 << 30) / ndir, "f16x3_split_dg: too many rows or columns");
+    const int Rp = b200asr_f16x3_padded_k(rows), Kp = b200asr_f16x3_padded_k(cols);
+    B200_CUDA(cudaFuncSetAttribute(f16_split_dg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM));
+    dim3 grid(Rp / F_CK, Kp / F_CK, ndir);
+    f16_split_dg_kernel<<<grid, 256, DG_SMEM, (cudaStream_t)stream>>>(g, rows, cols, Kp, Rp, (__half*)t_hi,
+                                                                      (__half*)t_lo, t_sinv, (__half*)r_hi,
+                                                                      (__half*)r_lo, r_sinv, colsum);
+    B200_LAUNCH_CHECK("f16_split_dg_kernel");
     return B200_OK;
 }
 

@@ -75,6 +75,7 @@ SIGNATURES = {
     "b200asr_f16x3_padded_k": (c_int, [c_int]),
     "b200asr_f16x3_split_rows": (c_int, [_P, c_longlong, c_int, c_int, _P, _P, _P, _P]),
     "b200asr_f16x3_split_cols": (c_int, [_P, c_longlong, c_longlong, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
+    "b200asr_f16x3_split_dg": (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "b200asr_gemm_f16x3": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_size_t,
                                    _P]),
     "b200asr_split_tf32": (c_int, [_P, _P, _P, c_longlong, _P]),

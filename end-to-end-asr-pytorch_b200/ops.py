@@ -175,6 +175,42 @@ def f16_split_t(x, cols, T, batches=1, ld=None, bstride=0, shift=0):
     return img, sinv
 
 
+def f16_split_dg(g, row_images=True):
+    """Gate gradient g[ndir, R, C] (contiguous) read once -> (per direction d the f16_split_t operand of g[d], the
+    f16_split operand of all directions side by side or None, column sums [ndir, C]).  The row operand's images are
+    [2, R, ndir * Kp] with direction d in columns [d * Kp, (d + 1) * Kp) (Kp = C padded to the scale chunk) and its
+    sinv [ndir * Kp // 128, R]; the column sums add per-128-row-tile partial sums in a fixed order (no atomics)."""
+    lib = L.load()
+    assert g.is_contiguous() and g.dim() == 3
+    ndir, R, C = g.shape
+    Rp, Kp = lib.b200asr_f16x3_padded_k(R), lib.b200asr_f16x3_padded_k(C)
+    timg = torch.empty((2, ndir, C, Rp), device=g.device, dtype=torch.float16)
+    tsinv = torch.empty((ndir, Rp // 128, C), device=g.device, dtype=torch.float32)
+    rimg = rsinv = None
+    if row_images:
+        rimg = torch.empty((2, R, ndir * Kp), device=g.device, dtype=torch.float16)
+        rsinv = torch.empty((ndir * Kp // 128, R), device=g.device, dtype=torch.float32)
+    part = torch.empty((Rp // 128, ndir * C), device=g.device, dtype=torch.float32)
+    nbytes = 4 * ndir * (R * C + C * Rp + (R * Kp if row_images else 0)) + 4 * part.numel()
+    with L.timed("f16_split_dg", nbytes):
+        L.check(lib.b200asr_f16x3_split_dg(L.ptr(g), ndir, R, C, L.ptr(timg[0]), L.ptr(timg[1]), L.ptr(tsinv),
+                                           L.ptr(rimg[0] if row_images else None),
+                                           L.ptr(rimg[1] if row_images else None), L.ptr(rsinv), L.ptr(part),
+                                           L.stream()), "f16x3_split_dg")
+    return ([(timg[:, d], tsinv[d]) for d in range(ndir)], (rimg, rsinv) if row_images else None,
+            part.sum(0).view(ndir, C))
+
+
+def f16_split_cat_t(ws, Kp):
+    """f16_split operand of [w_0^T | w_1^T | ...] (w_d [C, N]) with each block's C columns zero-padded to Kp: the B
+    operand that pairs with f16_split_dg's row images, so that sum_d g_d . w_d is one contraction over all blocks."""
+    C, N = ws[0].shape
+    wt = torch.zeros((N, len(ws), Kp), device=ws[0].device, dtype=torch.float32)
+    for d, w in enumerate(ws):
+        wt[:, d, :C] = w.t()
+    return f16_split(wt.view(N, len(ws) * Kp), N, len(ws) * Kp)
+
+
 def gemm_f16x3(a, b, bias=None, out=None, accumulate=False, permute_rows=False, name="gemm_f16_tn"):
     """out[M,N] (= or +=) A . B^T (+ bias[N]) for two f16x3 operands (f16_split / f16_split_t with the same Kp):
     fp32-class products on the fp16 tensor cores (csrc/gemm.cu).  permute_rows writes row m to (m%4)*(M/4) + m/4."""
@@ -379,6 +415,13 @@ class BiLSTMFn(Function):
         f16 = I % 4 == 0
         if f16:
             xt = f16_split_t(x, I, B * T)
+            # dG (d(loss)/d(pre-activation), unit-major columns) of both directions read once: its transposed images,
+            # its row images and its column sums (the bias gradient)
+            gts, grow, gsum = f16_split_dg(gates.view(ndir, B * T, 4 * H), row_images=need_dx)
+            if need_dx:
+                # dX = sum_d dG_d . W_d as one contraction over both directions
+                gemm_f16x3(grow, f16_split_cat_t(w_ih_p, grow[0].shape[2] // ndir), out=dx2)
+                del grow
         else:
             xs = Split(x.view(B * T, I))
         grads = []
@@ -386,13 +429,9 @@ class BiLSTMFn(Function):
             g2 = gates[d].view(B * T, 4 * H)      # d(loss)/d(pre-activation), unit-major columns
             hd = out[:, :, d * H:(d + 1) * H]
             if f16:
-                # dX = dG . W on the row images of dG and W^T; dW_ih = dG^T . X and dW_hh = dG^T . h_prev on transposed
-                # images (h_prev's written shifted by one step per utterance, zero at the sequence ends); rows written
-                # through the gate permutation by the epilogue.
-                if need_dx:
-                    gemm_f16x3(f16_split(g2, B * T, 4 * H), f16_split(w_ih_p[d].t().contiguous(), I, 4 * H), out=dx2,
-                               accumulate=(d > 0))
-                gt = f16_split_t(g2, 4 * H, B * T)
+                # dW_ih = dG^T . X and dW_hh = dG^T . h_prev on transposed images (h_prev's written shifted by one step
+                # per utterance, zero at the sequence ends); rows written through the gate permutation by the epilogue.
+                gt = gts[d]
                 dw_ih = gemm_f16x3(gt, xt, permute_rows=True, name="gemm_f16_nt")
                 ht = f16_split_t(hd, H, T, batches=B, ld=ndir * H, bstride=T * ndir * H, shift=(-1 if d == 0 else 1))
                 dw_hh = gemm_f16x3(gt, ht, permute_rows=True, name="gemm_f16_nt")
@@ -414,7 +453,7 @@ class BiLSTMFn(Function):
                 dw_hh.index_copy_(0, perm, mm3(dG.t(), Split(hprev.view(B * T, H))))
                 del dG, hprev
             db = torch.empty((4 * H,), device=dev, dtype=torch.float32)
-            db.index_copy_(0, perm, g2.sum(0))
+            db.index_copy_(0, perm, gsum[d] if f16 else g2.sum(0))
             grads += [dw_ih, dw_hh, db, db.clone()]
         return (dx2.view(B, T, I) if need_dx else None, None, *grads, *ctx.tail)
 

@@ -274,6 +274,12 @@ B200ASR_API int b200asr_tf32_residual(const float* x, float* lo, long long n, b2
  *   _split_rows: K-major x (element (row, k) at x[row * ld + k]; K, ld multiples of 4, 16-byte aligned).
  *   _split_cols: MN-major x, transposed: image row = column c, image column r = b T + t, element at
  *     x[b * bstride + (t + shift) * ld + c], zero where t + shift is outside [0, T) (h_prev of a direction).
+ *   _split_dg: the gate gradient of a BiLSTM layer, g[ndir][rows][cols] (contiguous; cols a multiple of 4, 16-byte
+ *     aligned), read once: per direction d the _split_cols operand of g[d] (t_hi / t_lo [ndir][cols][Rp], t_sinv
+ *     [ndir][Rp / 128][cols], Rp = padded rows); if r_hi / r_lo / r_sinv are given (all or none), one _split_rows
+ *     operand of all directions side by side (images [rows][ndir Kp], Kp = padded cols, direction d in columns
+ *     [d Kp, (d + 1) Kp); r_sinv [ndir Kp / 128][rows]); and colsum[Rp / 128][ndir][cols], the column sums of each
+ *     128-row tile.  Images and scales are bit-identical to the two single-image passes on the same data.
  *   b200asr_gemm_f16x3:  C[M,N] (+)= sum_k A[m][k] B[n][k] (+ bias[N]) over the two operands' images (same Kp):
  *     hi.hi + hi.lo + lo.hi per 16 k on the tensor cores, each 128-k chunk folded with its scales into an fp32
  *     register sum; ldc, accumulate, permute_rows (row m -> (m % 4) * (M / 4) + m / 4) and the split-K workspace
@@ -283,6 +289,8 @@ B200ASR_API int b200asr_f16x3_split_rows(const float* x, long long ld, int rows,
                              b200asr_stream stream);
 B200ASR_API int b200asr_f16x3_split_cols(const float* x, long long ld, long long bstride, int shift, int T, int batches,
                              int cols, void* hi, void* lo, float* sinv, b200asr_stream stream);
+B200ASR_API int b200asr_f16x3_split_dg(const float* g, int ndir, int rows, int cols, void* t_hi, void* t_lo, float* t_sinv,
+                           void* r_hi, void* r_lo, float* r_sinv, float* colsum, b200asr_stream stream);
 B200ASR_API int b200asr_gemm_f16x3(const void* a_hi, const void* a_lo, const float* a_sinv, const void* b_hi, const void* b_lo,
                        const float* b_sinv, const float* bias, float* C, int M, int N, int Kp, int ldc, int accumulate,
                        int permute_rows, void* workspace, size_t workspace_bytes, b200asr_stream stream);

@@ -2,9 +2,9 @@
 (input projection, input gradient and the transposed weight copy it needs, dW_ih, shifted dW_hh), with the share of
 the fp32-class ceiling, for both paths: 3xTF32 runs three TF32 passes, so its ceiling is a third of the data-sheet dense
 TF32 rate (495 / 3 = 165 TFLOP/s on an H100 SXM at 700 W); f16x3 runs three fp16 products, a third of the data-sheet
-dense fp16 rate (989 / 3 = 330 TFLOP/s), and its operand preparation passes (f16_split, memory-bound) are timed as
-calls of their own.  The step runs these contractions on f16x3; the 3xTF32 rows (through ops.gemm_tn / gemm_nn /
-gemm_nt) are a comparison of the two kernels at the same shapes, not calls the step makes.  Prints the card name and
+dense fp16 rate (989 / 3 = 330 TFLOP/s), and its operand preparation passes (f16_split, and f16_split_dg: one pass
+over dG of both directions; memory-bound) are timed as calls of their own.  The step runs these contractions on f16x3;
+the 3xTF32 rows (through ops.gemm_tn / gemm_nn / gemm_nt) are a comparison of the two kernels at the same shapes, not calls the step makes.  Prints the card name and
 power limit of the run.  QUICK=1 times layer 3 only."""
 import importlib, os, subprocess, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -65,21 +65,24 @@ for li, (rows, I) in ((i, l) for i, l in enumerate(LAYERS) if l in layers):
         if "nn" not in name:                     # the step runs the tn form of dX; nn is listed for comparison
             step_ms += 2 * ms
             step_tf += 2 * 2.0 * M * N * K / 1e12
-    # f16x3: the images one direction makes (x's and X^T's are made once per layer and shared by both directions:
-    # counted at half weight per direction)
-    xi, wi, gi = ops.f16_split(x, rows, I), ops.f16_split(w, 4 * H, I), ops.f16_split(g, rows, 4 * H)
-    wti, gt = ops.f16_split(wt, I, 4 * H), ops.f16_split_t(g, 4 * H, rows)
+    # f16x3 as the step runs it: weight 1 = once per direction, 0.5 = once per layer (x's and X^T's images, the one
+    # pass over dG of both directions, the dX contraction over both directions)
+    g2 = torch.stack([g, g])
+    xi, wi = ops.f16_split(x, rows, I), ops.f16_split(w, 4 * H, I)
+    gts, grow, _ = ops.f16_split_dg(g2, row_images=li > 0)
+    gt, wti = gts[0], None
     xt = ops.f16_split_t(x, I, rows)
     ht = ops.f16_split_t(h, H, T, batches=B, ld=2 * H, bstride=T * 2 * H, shift=-1)
     fcalls = [("L%d f16 split x (per layer)" % li, 0, 0, 0, 0.5, lambda: ops.f16_split(x, rows, I)),
               ("L%d f16 split W" % li, 0, 0, 0, 1, lambda: ops.f16_split(w, 4 * H, I)),
-              ("L%d f16 input projection" % li, rows, 4 * H, I, 1, lambda: ops.gemm_f16x3(xi, wi))]
+              ("L%d f16 input projection" % li, rows, 4 * H, I, 1, lambda: ops.gemm_f16x3(xi, wi)),
+              ("L%d f16 dG prep (per layer)" % li, 0, 0, 0, 0.5, lambda: ops.f16_split_dg(g2, row_images=li > 0))]
     if li > 0:
-        fcalls += [("L%d f16 split dG" % li, 0, 0, 0, 1, lambda: ops.f16_split(g, rows, 4 * H)),
-                   ("L%d f16 split W^T (copy incl.)" % li, 0, 0, 0, 1, lambda: ops.f16_split(w.t().contiguous(), I, 4 * H)),
-                   ("L%d f16 dX" % li, rows, I, 4 * H, 1, lambda: ops.gemm_f16x3(gi, wti))]
-    fcalls += [("L%d f16 split dG^T" % li, 0, 0, 0, 1, lambda: ops.f16_split_t(g, 4 * H, rows)),
-               ("L%d f16 split X^T (per layer)" % li, 0, 0, 0, 0.5, lambda: ops.f16_split_t(x, I, rows)),
+        wti = ops.f16_split_cat_t([w, w], grow[0].shape[2] // 2)
+        fcalls += [("L%d f16 split [W^T|W^T] (per layer)" % li, 0, 0, 0, 0.5,
+                    lambda: ops.f16_split_cat_t([w, w], grow[0].shape[2] // 2)),
+                   ("L%d f16 dX (per layer)" % li, rows, I, 8 * H, 0.5, lambda: ops.gemm_f16x3(grow, wti))]
+    fcalls += [("L%d f16 split X^T (per layer)" % li, 0, 0, 0, 0.5, lambda: ops.f16_split_t(x, I, rows)),
                ("L%d f16 dW_ih" % li, 4 * H, I, rows, 1, lambda: ops.gemm_f16x3(gt, xt, permute_rows=True)),
                ("L%d f16 split h_prev^T (shifted)" % li, 0, 0, 0, 1,
                 lambda: ops.f16_split_t(h, H, T, batches=B, ld=2 * H, bstride=T * 2 * H, shift=-1)),
@@ -92,8 +95,8 @@ for li, (rows, I) in ((i, l) for i, l in enumerate(LAYERS) if l in layers):
         else:
             tf = 2.0 * M * N * K / ms / 1e9
             print("%-34s %6d %5d %5d %8.3f %8.1f %6.1f%%" % (name, M, N, K, ms, tf, 100 * tf / CEILING_F16), flush=True)
-            f16_ms += 2 * ms
-    del x, w, g, h, wlo, wt, wtlo, xi, wi, gi, wti, gt, xt, ht
+            f16_ms += 2 * wgt * ms
+    del x, w, g, g2, h, wlo, wt, wtlo, xi, wi, wti, gts, grow, gt, xt, ht
 print("sum over both directions: %.1f ms for %.2f TFLOP = %.1f TFLOP/s (%.1f%% of the %.0f TFLOP/s ceiling)"
       % (step_ms, step_tf, step_tf / step_ms * 1e3, 100 * step_tf / step_ms * 1e3 / CEILING, CEILING))
 print("f16x3, both directions: GEMMs %.1f ms = %.1f TFLOP/s (%.1f%% of the %.0f TFLOP/s ceiling), preparation passes "
