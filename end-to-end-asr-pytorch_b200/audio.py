@@ -136,17 +136,32 @@ class FbankFrontEnd(torch.nn.Module):
 
     @torch.no_grad()
     def forward(self, wave, wave_len, t_max=None, return_fbank=False):
-        """wave [B, N_max] fp32 CUDA (zero padded), wave_len [B] (any int tensor / list).
-        Returns (feat [B, T_max, D], feat_len [B] int64 on the same device)."""
+        """wave [B, N_max] fp32 or int16 CUDA (zero padded), wave_len [B] samples (any int tensor / list).
+        Returns (feat [B, t_max, D], feat_len [B] int64 on the same device) (+ the log-mel fbank [B, t_max, n_mel]
+        with return_fbank).  t_max defaults to the frame count of N_max samples.
+
+        An utterance is its first min(frames(wave_len[b]), t_max) frames: a smaller t_max truncates it (feat_len
+        is then t_max, and the CMVN statistics and deltas see only the kept frames).  Lengths known on the host (a
+        list or a CPU tensor) must lie in [0, N_max], else ValueError; lengths already on the device are clamped
+        to [0, N_max] by the kernel, so no sample outside a row is read."""
         lib = L.load()
         if self.window.device != wave.device:
             self.to(wave.device)
         pcm16 = wave.dtype == torch.int16            # 16-bit PCM: converted on the fly by the kernel (sample / 32768)
         wave = wave.contiguous() if pcm16 else wave.to(torch.float32).contiguous()
         B, N = wave.shape
+        if not (torch.is_tensor(wave_len) and wave_len.is_cuda):
+            host = torch.as_tensor(wave_len)
+            if host.numel() and (int(host.min()) < 0 or int(host.max()) > N):
+                raise ValueError("wave_len must lie in [0, %d] (the padded length), got %s" % (N, host.tolist()))
         wl = torch.as_tensor(wave_len).to(device=wave.device, dtype=torch.int32).contiguous()
         if t_max is None:
             t_max = self.num_frames(N)
+        if t_max == 0:   # no frame to compute (e.g. one utterance shorter than a window): empty, launch nothing
+            fb = torch.zeros((B, 0, self.num_mel), device=wave.device)
+            feat = fb if self.delta_order == 0 and not self.apply_cmvn else fb.new_zeros((B, 0, self.feat_dim))
+            n = torch.zeros(B, device=wave.device, dtype=torch.int64)
+            return (feat, n, fb) if return_fbank else (feat, n)
         fb = torch.empty((B, t_max, self.num_mel), device=wave.device, dtype=torch.float32)
         nfr = torch.empty(B, device=wave.device, dtype=torch.int32)
         # algorithmic bytes (SURVEY.md 8(d)): read the waveform once, write the mel features once
@@ -200,8 +215,8 @@ class FileTransform(torch.nn.Module):
         self.frontend = frontend
         self.device = device
 
-    def batch(self, wave, wave_len, t_max=None):
-        return self.frontend(wave, wave_len, t_max)
+    def batch(self, wave, wave_len, t_max=None, return_fbank=False):
+        return self.frontend(wave, wave_len, t_max, return_fbank)
 
     def forward(self, filepath):
         wave, sr = load_wav(filepath)

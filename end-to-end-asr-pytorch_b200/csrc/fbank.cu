@@ -74,6 +74,14 @@ __device__ __forceinline__ void fft256_pass(const float2* __restrict__ x, float2
     __syncwarp();
 }
 
+// Frames of utterance b: its samples are the first clamp(wave_len, 0, n_max) of its row, and at most t_max frames are
+// kept, so no frame reads past the row and n_frames never exceeds the rows that were written.
+__device__ __forceinline__ int utt_frames(const FbankParams& p, int b) {
+    const int n = min(max(p.wave_len[b], 0), p.n_max);
+    const int m = (n >= p.win) ? 1 + (n - p.win) / p.shift : 0;
+    return min(m, p.t_max);
+}
+
 __global__ void __launch_bounds__(FB_WARPS * 32) fbank_kernel(FbankParams p) {
     __shared__ float2 s_w512[FB_NFFT];
     __shared__ float s_window[FB_NFFT];
@@ -95,12 +103,8 @@ __global__ void __launch_bounds__(FB_WARPS * 32) fbank_kernel(FbankParams p) {
         s_mcount[k] = p.mel_count[k];
         s_moff[k] = p.mel_off[k];
     }
-    if (blockIdx.x == 0) {
-        for (int b = tid; b < p.B; b += blockDim.x) {
-            const int n = p.wave_len[b];
-            p.n_frames[b] = (n >= p.win) ? 1 + (n - p.win) / p.shift : 0;
-        }
-    }
+    if (blockIdx.x == 0)
+        for (int b = tid; b < p.B; b += blockDim.x) p.n_frames[b] = utt_frames(p, b);
     __syncthreads();
 
     float* sA = s_buf[warp][0];
@@ -111,8 +115,7 @@ __global__ void __launch_bounds__(FB_WARPS * 32) fbank_kernel(FbankParams p) {
     for (long long item = (long long)blockIdx.x * FB_WARPS + warp; item < total; item += wstride) {
         const int b = (int)(item / p.t_max);
         const int f = (int)(item - (long long)b * p.t_max);
-        const int n = p.wave_len[b];
-        const int m = (n >= p.win) ? 1 + (n - p.win) / p.shift : 0;
+        const int m = utt_frames(p, b);
         float* o = p.out + item * p.n_mel;
         if (f >= m) {  // padded frame
             for (int i = lane; i < p.n_mel; i += 32) o[i] = 0.f;
@@ -261,7 +264,7 @@ __global__ void __launch_bounds__(DC_COLS* DC_ROWS) delta_stats_kernel(DeltaPara
     extern __shared__ float s_fb[];
     const int b = blockIdx.y, ch = blockIdx.x;
     const int D = p.n_mel * (p.order + 1);
-    const int m = p.n_frames[b];
+    const int m = min(max(p.n_frames[b], 0), p.t_max);   // the utterance is its first m rows: no read past them
     const float* fb = p.fb + (long long)b * p.t_max * p.n_mel;
     const int r = threadIdx.x / DC_COLS, cl = threadIdx.x % DC_COLS;
     const int t0 = ch * DC_TCHUNK, t1 = min(m, t0 + DC_TCHUNK);
@@ -302,7 +305,7 @@ __global__ void __launch_bounds__(DC_COLS* DC_ROWS) delta_norm_kernel(DeltaParam
     extern __shared__ float s_fb[];
     const int b = blockIdx.y, ch = blockIdx.x;
     const int D = p.n_mel * (p.order + 1);
-    const int m = p.n_frames[b];
+    const int m = min(max(p.n_frames[b], 0), p.t_max);   // same clamp as delta_stats_kernel: mchunks <= nchunk
     const float* fb = p.fb + (long long)b * p.t_max * p.n_mel;
     float* out = p.out + (long long)b * p.t_max * D;
     const int r = threadIdx.x / DC_COLS, cl = threadIdx.x % DC_COLS;

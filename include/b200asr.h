@@ -44,7 +44,9 @@ B200ASR_API int b200asr_device_sm_count(void);
  * window).  wave [B, n_max] (zero padded), wave_len [B] samples.  window [win_size] and the sparse mel
  * filters (filter i covers FFT bins mel_start[i] .. +mel_count[i], weights at mel_w[mel_off[i] ..]) are
  * caller-built tables.  fbank [B, t_max, n_mel] (frames >= n_frames[b] are zeroed), n_frames [B] (int32 out)
- * = 1 + (len - win_size) / win_shift (snip_edges=True).  n_fft must be 512.                               */
+ * = min(1 + (n - win_size) / win_shift, t_max) with n = clamp(wave_len[b], 0, n_max) (snip_edges=True; 0 when
+ * n < win_size): an utterance is its first min(frames, t_max) frames, and no sample at or beyond n_max of its row is
+ * read whatever wave_len says.  n_fft must be 512.                                                          */
 B200ASR_API int b200asr_fbank_fwd(const float* wave, const int* wave_len, int B, int n_max, int win_size, int win_shift,
                       int n_fft, float preemph, int remove_dc, const float* window, int n_mel,
                       const int* mel_start, const int* mel_count, const int* mel_off, const float* mel_w,
@@ -61,7 +63,8 @@ B200ASR_API int b200asr_fbank_fwd_pcm16(const short* pcm, const int* wave_len, i
 /* ---- K2+K3: delta / delta-delta + per-utterance CMVN + channel-major interleave ---------------------------
  * replaces src/audio.py:51-54,57-77 (Delta), :25-27 (CMVN, unbiased std, eps added to std), :85-89
  * (Postprocess).  feat [B, t_max, n_mel*(delta_order+1)], rows >= n_frames[b] are zero (pad_sequence,
- * src/data.py:39).                                                                                          */
+ * src/data.py:39).  Utterance b is its first m = clamp(n_frames[b], 0, t_max) fbank rows: the CMVN statistics
+ * cover exactly those m frames, the delta taps see zeros beyond them, and rows at or beyond m are never read.     */
 B200ASR_API size_t b200asr_delta_cmvn_workspace_bytes(int B, int t_max, int n_mel, int delta_order);
 B200ASR_API int b200asr_delta_cmvn_fwd(const float* fbank, const int* n_frames, int B, int t_max, int n_mel,
                                        int delta_order, int delta_window, int apply_cmvn, float cmvn_eps,

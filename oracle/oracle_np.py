@@ -77,6 +77,28 @@ def fbank(wave, sample_freq=16000.0, num_mel_bins=40, frame_length=25.0, frame_s
     return np.log(np.maximum(mel, dtype(FLT_EPS))).astype(dtype)             # kaldi.py:633
 
 
+def fbank_tables(wave, window, mel, win, shift, remove_dc=True, preemph=0.97, use_log=True, log_floor=FLT_EPS):
+    """float64 fbank on given tables: window [win] and dense mel weights [n_mel, n_fft//2 + 1], taken at the values
+    passed (the kernel's fp32 tables; torchaudio builds its mel weights in fp32 even for a float64 waveform), every
+    other step in float64.  wave [N] -> [m, n_mel], m = 1 + (N - win) // shift (snip_edges); log of
+    max(mel, log_floor) when use_log, else the linear mel energies."""
+    x = np.asarray(wave, np.float64)
+    mel = np.asarray(mel, np.float64)
+    n_fft = 2 * (mel.shape[1] - 1)
+    if x.shape[0] < win:
+        return np.zeros((0, mel.shape[0]))
+    m = 1 + (x.shape[0] - win) // shift
+    fr = x[np.arange(win)[None, :] + shift * np.arange(m)[:, None]]
+    if remove_dc:
+        fr = fr - fr.mean(axis=1, keepdims=True)
+    if preemph != 0.0:
+        fr = fr - float(preemph) * np.concatenate([fr[:, :1], fr[:, :-1]], axis=1)
+    fr = fr * np.asarray(window, np.float64)[None, :win]
+    spec = np.abs(np.fft.rfft(fr, n=n_fft, axis=1)) ** 2
+    e = spec @ mel.T
+    return np.log(np.maximum(e, float(log_floor))) if use_log else e
+
+
 def delta_filters(order, window):
     # src/audio.py:57-77
     scales = [[1.0]]
@@ -114,11 +136,11 @@ def delta_cmvn(fb, order=2, window=2, apply_cmvn=True, eps=1e-10, dtype=np.float
                 acc = acc + filt[o, tap] * xp[tap:tap + m]
         chans.append(acc)
     x = np.stack(chans, 0)                                                   # [C, m, F]
-    if apply_cmvn:
+    if apply_cmvn and m > 0:
         mean = x.mean(axis=1, keepdims=True)
         std = x.std(axis=1, ddof=1, keepdims=True) if m > 1 else np.full_like(mean, np.nan)
         x = (x - mean) / (dtype(eps) + std)
-    return np.transpose(x, (1, 0, 2)).reshape(m, -1).astype(dtype)
+    return np.transpose(x, (1, 0, 2)).reshape(m, F * (order + 1)).astype(dtype)
 
 
 # ------------------------------------------------------------------------------------------------ LSTM

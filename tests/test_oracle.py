@@ -64,6 +64,57 @@ def test_delta_filters():
     assert np.allclose(f[2], [.04, .04, .01, -.04, -.1, -.04, .01, .04, .04])
 
 
+@pytest.mark.parametrize("window_type", ["hanning", "hamming", "povey", "rectangular", "blackman"])
+@pytest.mark.parametrize("opts", [
+    {}, dict(use_log_fbank=False), dict(remove_dc_offset=False), dict(preemphasis_coefficient=0.0),
+    dict(sample_frequency=8000.0, frame_length=50.0, frame_shift=12.5, low_freq=0.0, high_freq=-200.0),
+    dict(sample_frequency=22050.0, frame_length=20.0), dict(num_mel_bins=128, frame_length=32.0, frame_shift=1.0),
+], ids=["default", "linear", "no-dc", "no-preemph", "8k-neg-high", "22k", "128mel-512"])
+def test_fbank_tables_matches_float64_kaldi(pkg, window_type, opts):
+    """oracle_np.fbank_tables on the tables torchaudio itself uses for a float64 waveform (its fp32 mel weights, its
+    float64 window) agrees with kaldi.fbank at float64 level, for every window and option the front end accepts."""
+    import torchaudio.compliance.kaldi as kaldi
+    o = dict(sample_frequency=16000.0, frame_length=25.0, frame_shift=10.0, low_freq=20.0, high_freq=0.0,
+             num_mel_bins=40, use_log_fbank=True, remove_dc_offset=True, preemphasis_coefficient=0.97)
+    o.update(opts)
+    sr = o["sample_frequency"]
+    rng = np.random.default_rng(len(window_type) + len(opts))
+    x = 0.3 + 0.1 * rng.standard_normal(int(0.4 * sr))
+    x[: int(0.1 * sr)] *= 1e-3
+    ref = kaldi.fbank(torch.from_numpy(x)[None], window_type=window_type, dither=0.0, **o).numpy()
+    win, shift = int(sr * o["frame_length"] * 0.001), int(sr * o["frame_shift"] * 0.001)
+    window = kaldi._feature_window_function(window_type, win, 0.42, "cpu", torch.float64).numpy()
+    mel = pkg.audio.mel_filterbank(o["num_mel_bins"], 512, sr, o["low_freq"], o["high_freq"]).numpy()
+    got = onp.fbank_tables(x, window, mel, win, shift, o["remove_dc_offset"], o["preemphasis_coefficient"],
+                           o["use_log_fbank"])
+    assert ref.dtype == np.float64 and got.shape == ref.shape
+    scale = 1.0 if o["use_log_fbank"] else float(np.abs(ref).max())
+    assert float(np.abs(got - ref).max()) / scale < 1e-10
+    # the kernel's fp32 window table moves the log-mel by up to ~2e-4 on the quiet segment: why the oracle takes the
+    # kernel's own tables instead of building its own
+    w32 = pkg.audio.window_function(window_type, win).numpy()
+    got32 = onp.fbank_tables(x, w32, mel, win, shift, o["remove_dc_offset"], o["preemphasis_coefficient"],
+                             o["use_log_fbank"])
+    assert float(np.abs(got32 - ref).max()) / scale < 1e-3
+
+
+@pytest.mark.parametrize("order,window", [(0, 2), (1, 1), (1, 16), (2, 2), (2, 8)])
+def test_delta_cmvn_matches_float64_conv(order, window):
+    """delta_cmvn up to 33 taps against a zero-padded float64 conv1d of the same filters, with and without CMVN."""
+    rng = np.random.default_rng(order * 100 + window)
+    fb = rng.standard_normal((70, 6)) + np.arange(6)
+    filt = onp.delta_filters(order, window)
+    assert filt.shape == (order + 1, 2 * order * window + 1)
+    pad = (filt.shape[1] - 1) // 2
+    x = torch.from_numpy(fb.T.copy())[:, None, :]                              # [F, 1, m]
+    y = torch.nn.functional.conv1d(x, torch.from_numpy(filt)[:, None, :], padding=pad)   # [F, C, m]
+    raw = y.permute(2, 1, 0).reshape(70, -1).numpy()                           # channel-major [m, C*F]
+    assert np.abs(onp.delta_cmvn(fb, order, window, apply_cmvn=False) - raw).max() < 1e-12
+    cm = (raw - raw.mean(0)) / (1e-10 + raw.std(0, ddof=1))
+    assert np.abs(onp.delta_cmvn(fb, order, window, apply_cmvn=True) - cm).max() < 1e-12
+    assert onp.delta_cmvn(fb[:0], order, window).shape == (0, 6 * (order + 1))
+
+
 # ------------------------------------------------------------------------------------------- CTC
 def test_ctc_np_matches_aten_cases():
     g = load_golden("ctc_cases.npz")
