@@ -54,17 +54,11 @@ struct LstmParams {
     float* xbuf;         // exchange buffers
     unsigned* counters;  // [ndir][nbg][NH]
     int* err_flag;
-    long long* trace;    // optional [T][16] clock64 stamps of CTA 0 / group 0 (debug; NULL in production)
     int B, T, H, ndir, UB, Bc, nub, nbg, NH, R;
     int b0, Bend;        // this launch covers batch rows [b0, Bend) of the B rows the tensors hold
-    int flags;           // debug switches: bit 2 = first-generation MMA loops (every warp polls, compiler-pipelined),
-                         // bit 3 = clock64 trace of the backward instead of the forward kernel
     int mma;             // 1: tensor-core (3xTF32 mma.sync) step GEMMs, see the *_mma kernels
-    int form;            // loop form of the mma.sync kernels, LstmVariant::form
+    int form;            // loop form of the mma.sync forward, LstmVariant::form
 };
-
-#define LSTM_TRACE(slot) \
-    do { if (p.trace && blockIdx.x == 0) p.trace[(size_t)step * 16 + (slot)] = clock64(); } while (0)
 
 __device__ __forceinline__ void spin_until(const unsigned* ctr, unsigned target, int* err_flag) {
     const long long t0 = clock64();
@@ -121,22 +115,19 @@ __global__ void lstm_pack_kernel(const float* __restrict__ w, float* __restrict_
 __device__ __forceinline__ void control_loop(const LstmParams& p, int T, unsigned nub, uint64_t* done, uint64_t* full,
                                              unsigned* ctr, const float* src_even, const float* src_odd, float* dst,
                                              const uint32_t* src_off, const uint32_t* dst_off,
-                                             const uint32_t* chunk_bytes, bool trace_me) {
+                                             const uint32_t* chunk_bytes) {
     for (int step = 0; step + 1 < T; ++step) {
         mbar_wait(done, (uint32_t)(step & 1));          // every compute warp of the group finished `step`
-        if (trace_me) LSTM_TRACE(8);
-        __threadfence();                                // their global stores (made visible to me through the
-        if (trace_me) LSTM_TRACE(9);                    // mbarrier) are ordered before the release
+        // their global stores (made visible to me through the mbarrier) are ordered before the release
+        __threadfence();
         red_release_add_u32(ctr, 1u);
         spin_until(ctr, (unsigned)(step + 1) * nub, p.err_flag);
-        if (trace_me) LSTM_TRACE(10);
         fence_proxy_async();
         const float* src = (step & 1) ? src_odd : src_even;
         for (int c = 0; c < LSTM_NCHUNK; ++c) {
             mbar_expect_tx(&full[c], chunk_bytes[c]);
             if (chunk_bytes[c]) bulk_g2s(dst + dst_off[c], src + src_off[c], chunk_bytes[c], &full[c]);
         }
-        if (trace_me) LSTM_TRACE(11);
     }
 }
 
@@ -193,14 +184,12 @@ __device__ __forceinline__ void fwd_group(const LstmParams& p, int g, int gt, in
     const int bglob0 = p.b0 + bg * p.Bc + g * Bh + bl0;
     const size_t half_elems = (size_t)H * Bh;
     const int chunk_stride = KC * Bh + LSTM_CHUNK_PAD;   // padded so the 4 chunks start in different banks
-    const bool trc = (g == 0 && gt == 0);
     float c_reg[RL];
 #pragma unroll
     for (int i = 0; i < RL; ++i) c_reg[i] = 0.f;
 
     for (int step = 0; step < T; ++step) {
         const int tt = dir ? (T - 1 - step) : step;
-        if (trc) LSTM_TRACE(0);
         float4 gx[RL];
 #pragma unroll
         for (int i = 0; i < RL; ++i) {
@@ -228,7 +217,6 @@ __device__ __forceinline__ void fwd_group(const LstmParams& p, int g, int gt, in
 #pragma unroll
             for (int c = 0; c < LSTM_NCHUNK; ++c) mbar_wait(&full[c], (uint32_t)((step - 1) & 1));
             __syncwarp();
-            if (trc) LSTM_TRACE(1);
             if (has_tile) {
                 const float4* hp = reinterpret_cast<const float4*>(hsg + (size_t)kq * chunk_stride + bo * R);
                 const float4* wp = Ws + (size_t)kq * KC * UB + u;
@@ -277,7 +265,6 @@ __device__ __forceinline__ void fwd_group(const LstmParams& p, int g, int gt, in
 #pragma unroll
                     for (int q = 0; q < 4; ++q) unpack2(accp[rp][q], acc[2 * rp][q], acc[2 * rp + 1][q]);
             }
-            if (trc) LSTM_TRACE(3);
             if (p.NH == 2) {             // hand the FMA pipes to the other group
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&turn[1 - g]);
@@ -292,7 +279,6 @@ __device__ __forceinline__ void fwd_group(const LstmParams& p, int g, int gt, in
                     v += __shfl_xor_sync(0xffffffffu, v, 16);
                     acc[i][q] = v;
                 }
-            if (trc) LSTM_TRACE(4);
         }
         float hq[RL], cq[RL];
         float4 gq[RL];
@@ -321,7 +307,6 @@ __device__ __forceinline__ void fwd_group(const LstmParams& p, int g, int gt, in
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(done);
-            if (trc) LSTM_TRACE(5);
         }
 #pragma unroll
         for (int i = 0; i < RL; ++i) {
@@ -384,7 +369,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_fwd_kernel(LstmParams 
             }
             control_loop(p, T, (unsigned)p.nub, &done[g], &full[g * LSTM_NCHUNK], ctr0 + g,
                          xb + ((size_t)g * 2 + 0) * half_elems, xb + ((size_t)g * 2 + 1) * half_elems,
-                         hs + (size_t)g * hs_half, soff, doff, bytes, g == 0);
+                         hs + (size_t)g * hs_half, soff, doff, bytes);
         }
         return;
     }
@@ -646,7 +631,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_bwd_kernel(LstmParams 
             control_loop(p, T, (unsigned)nub, &done[g], &full[g * LSTM_NCHUNK], ctr0 + g,
                          xb + (((size_t)g * 2 + 0) * nub + ub) * inbox_elems,
                          xb + (((size_t)g * 2 + 1) * nub + ub) * inbox_elems, inbox + (size_t)g * inbox_elems, off, off,
-                         bytes, false);
+                         bytes);
         }
         return;
     }
@@ -759,12 +744,10 @@ __device__ __forceinline__ void fwd_group_mma(const LstmParams& p, int g, int gt
     const int chunk_stride = KC * 16 + LSTM_CHUNK_PAD;
     // where my two h values go in the NEXT step's A operand: k = ug -> k-step ug/8, column ug%8
     const size_t pub_off = ((size_t)(ug >> 3) * 32 + gid * 4 + (ug & 3)) * 4 + 2 * ((ug >> 2) & 1);
-    const bool trc = (g == 0 && gt == 0);
     float c_reg[2] = {0.f, 0.f};
 
     for (int step = 0; step < T; ++step) {
         const int tt = dir ? (T - 1 - step) : step;
-        if (trc) LSTM_TRACE(0);
         float4 gx[2];
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
@@ -784,13 +767,11 @@ __device__ __forceinline__ void fwd_group_mma(const LstmParams& p, int g, int gt
             // for their exchanges at the same time; in alternation one group's exchange hides behind the other's MMAs
             if (g == 1) mbar_wait(&turn[1], (uint32_t)((step - 1) & 1));
             else if (step >= 2) mbar_wait(&turn[0], (uint32_t)(step & 1));
-            if (trc) LSTM_TRACE(2);
 #pragma unroll 1
             for (int c = 0; c < LSTM_NCHUNK; ++c) {
                 // every warp waits (also one without units): the wait is what keeps a warp from running a step
                 // ahead and arriving twice in one phase of the group's `done` barrier
                 mbar_wait(&full[c], (uint32_t)((step - 1) & 1));
-                if (trc && c == 0) LSTM_TRACE(1);
                 if (!has_pair) continue;
                 const float4* ap = reinterpret_cast<const float4*>(hsg + (size_t)c * chunk_stride) + lane;
                 const float4* wp = Wm + ((size_t)c * KSC * npairs + warp) * 32 + lane;
@@ -830,7 +811,6 @@ __device__ __forceinline__ void fwd_group_mma(const LstmParams& p, int g, int gt
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&turn[1 - g]);
-            if (trc) LSTM_TRACE(3);
         }
         float hq[2] = {0.f, 0.f}, cq[2] = {0.f, 0.f};
         float4 gq[2];
@@ -854,7 +834,6 @@ __device__ __forceinline__ void fwd_group_mma(const LstmParams& p, int g, int gt
                 *reinterpret_cast<float2*>(xbg + (size_t)(step & 1) * half_elems + pub_off) = make_float2(hq[0], hq[1]);
             __syncwarp();
             if (lane == 0) mbar_arrive(done);
-            if (trc) LSTM_TRACE(5);
         }
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
@@ -888,12 +867,10 @@ __device__ __forceinline__ void fwd_group_mma_v2(const LstmParams& p, int g, int
     const int brow[2] = {p.b0 + bg * p.Bc + g * 16 + gid, p.b0 + bg * p.Bc + g * 16 + gid + 8};
     const size_t half_elems = (size_t)H * 16;
     const size_t pub_off = ((size_t)(ug >> 3) * 32 + gid * 4 + (ug & 3)) * 4 + 2 * ((ug >> 2) & 1);
-    const bool trc = (g == 0 && gt == 0);
     float c_reg[2] = {0.f, 0.f};
 
     for (int step = 0; step < T; ++step) {
         const int tt = dir ? (T - 1 - step) : step;
-        if (trc) LSTM_TRACE(0);
         float4 gx[2];
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
@@ -906,10 +883,8 @@ __device__ __forceinline__ void fwd_group_mma_v2(const LstmParams& p, int g, int
             if (warp == 0) {
                 if (g == 1) mbar_wait(&turn[1], (uint32_t)((step - 1) & 1));
                 else if (step >= 2) mbar_wait(&turn[0], (uint32_t)(step & 1));
-                if (trc) LSTM_TRACE(2);
 #pragma unroll
                 for (int c = 0; c < LSTM_NCHUNK; ++c) mbar_wait(&full[c], (uint32_t)((step - 1) & 1));
-                if (trc) LSTM_TRACE(1);
             }
             named_bar_sync(3 + g, LSTM_GTHREADS);
             if (has_pair) {
@@ -966,7 +941,6 @@ __device__ __forceinline__ void fwd_group_mma_v2(const LstmParams& p, int g, int
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&turn[1 - g]);
-            if (trc) LSTM_TRACE(3);
         }
         float hq[2] = {0.f, 0.f}, cq[2] = {0.f, 0.f};
         float4 gq[2];
@@ -990,7 +964,6 @@ __device__ __forceinline__ void fwd_group_mma_v2(const LstmParams& p, int g, int
                 *reinterpret_cast<float2*>(xbg + (size_t)(step & 1) * half_elems + pub_off) = make_float2(hq[0], hq[1]);
             __syncwarp();
             if (lane == 0) mbar_arrive(done);
-            if (trc) LSTM_TRACE(5);
         }
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
@@ -1049,7 +1022,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_fwd_mma_kernel(LstmPar
             }
             control_loop(p, T, (unsigned)p.nub, &done[g], &full[g * LSTM_NCHUNK], ctr0 + g,
                          xb + ((size_t)g * 2 + 0) * half_elems, xb + ((size_t)g * 2 + 1) * half_elems,
-                         hs + (size_t)g * hs_half, soff, doff, bytes, g == 0);
+                         hs + (size_t)g * hs_half, soff, doff, bytes);
         }
         return;
     }
@@ -1089,14 +1062,11 @@ __device__ __forceinline__ void bwd_group_mma(const LstmParams& p, int g, int gt
         it_ok[j] = it_in[j] && it_row[j] < p.Bend;
     }
     float dc_reg[2] = {0.f, 0.f};
-    const bool lead = p.form == 0;
-    const bool trc = (g == 0 && gt == 0);
 
     for (int step = 0; step < T; ++step) {
         const int fstep = T - 1 - step;
         const int tt = dir ? (T - 1 - fstep) : fstep;
         const int tt_prev = dir ? tt + 1 : tt - 1;
-        if (trc) LSTM_TRACE(0);
         float4 gtv[2];
         float ct[2], cp[2], dh[2];
 #pragma unroll
@@ -1113,20 +1083,13 @@ __device__ __forceinline__ void bwd_group_mma(const LstmParams& p, int g, int gt
             }
         }
         if (step > 0) {
-            if (lead) {
-                // only warp 0 polls; the other warps park in a hardware barrier and leave their schedulers' issue
-                // slots to the other group's MMA loop
-                if (warp == 0) {
-#pragma unroll
-                    for (int c = 0; c < LSTM_NCHUNK; ++c) mbar_wait(&full[c], (uint32_t)((step - 1) & 1));
-                }
-                named_bar_sync(3 + g, LSTM_GTHREADS);
-            } else {
+            // only warp 0 polls; the other warps park in a hardware barrier and leave their schedulers' issue slots
+            // to the other group's MMA loop
+            if (warp == 0) {
 #pragma unroll
                 for (int c = 0; c < LSTM_NCHUNK; ++c) mbar_wait(&full[c], (uint32_t)((step - 1) & 1));
-                __syncwarp();
             }
-            if (trc) LSTM_TRACE(1);
+            named_bar_sync(3 + g, LSTM_GTHREADS);
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
                 if (it_in[j]) {
@@ -1164,18 +1127,13 @@ __device__ __forceinline__ void bwd_group_mma(const LstmParams& p, int g, int gt
                 d[0] = dg.x; d[4] = dg.y; d[8] = dg.z; d[12] = dg.w;
             }
         }
-        if (lead && warp == 0 && step + 1 < T) {                            // groups alternate on the tensor pipe
+        if (warp == 0 && step + 1 < T) {                                    // groups alternate on the tensor pipe
             if (g == 1) mbar_wait(&turn[1], (uint32_t)(step & 1));
             else if (step >= 1) mbar_wait(&turn[0], (uint32_t)((step - 1) & 1));
         }
         named_bar_sync(1 + g, LSTM_GTHREADS);                              // dG tile complete (and turn acquired)
         if (step + 1 < T) {
-            if (!lead) {
-                if (g == 1) mbar_wait(&turn[1], (uint32_t)(step & 1));
-                else if (step >= 1) mbar_wait(&turn[0], (uint32_t)((step - 1) & 1));
-            }
             float* outbase = xbg + (size_t)(step & 1) * nub * inbox_elems;
-            if (trc) LSTM_TRACE(2);
             const float4* ap = reinterpret_cast<const float4*>(dgs) + lane;
             for (int nb = warp; nb < NB; nb += LSTM_GTHREADS / 32) {
                 float d[4][3][4];
@@ -1222,13 +1180,11 @@ __device__ __forceinline__ void bwd_group_mma(const LstmParams& p, int g, int gt
                     *reinterpret_cast<float2*>(o + (size_t)8 * UB) = make_float2(v2, v3);
                 }
             }
-            if (trc) LSTM_TRACE(3);
             __syncwarp();
             if (lane == 0) {
                 mbar_arrive(&turn[1 - g]);
                 mbar_arrive(done);
             }
-            if (trc) LSTM_TRACE(5);
         }
     }
 }
@@ -1277,7 +1233,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_bwd_mma_kernel(LstmPar
             control_loop(p, T, (unsigned)nub, &done[g], &full[g * LSTM_NCHUNK], ctr0 + g,
                          xb + (((size_t)g * 2 + 0) * nub + ub) * inbox_elems,
                          xb + (((size_t)g * 2 + 1) * nub + ub) * inbox_elems, inbox + (size_t)g * inbox_elems, off, off,
-                         bytes, g == 0);
+                         bytes);
         }
         return;
     }
@@ -1332,13 +1288,9 @@ struct Plan {
     size_t smem_fwd, smem_bwd, pack_bytes, xbuf_fwd_bytes, xbuf_bwd_bytes;
 };
 
-#ifndef LSTM_UMMA_BWD_DEFAULT
-#define LSTM_UMMA_BWD_DEFAULT 1
-#endif
-static int g_lstm_flags = 0;  // experiment switches, see LstmParams::flags (set through the upper bits of the mode)
-static int g_lstm_mode = 0;   // 0: wgmma (lstm_umma.cu) when the shape allows, else mma.sync, else fp32 FMA;
-                              // 1: always the fp32-FMA kernels, 2: mma.sync with 6 instead of 12 accumulator chains
-                              // (measurement only), 3: never wgmma (the mma.sync generation, for A/B comparisons)
+static int g_lstm_mode = 0;        // 0: wgmma (lstm_umma.cu) when the shape allows, else mma.sync, else fp32 FMA;
+                                   // 1: always the fp32-FMA kernels; 3: never wgmma (the mma.sync generation)
+static bool g_lstm_strict = false; // debug mode 256: formal acquire after the wgmma forward's flag poll
 
 static int halves_for(int Bc) { return (Bc % 8 == 0) ? 2 : 1; }
 static int rows_for(int Bc) { return ((Bc / halves_for(Bc)) % 8 == 0) ? 8 : 4; }
@@ -1406,7 +1358,7 @@ static int plan_one(int B, int H, int ndir, Plan* out) {
                 best_mma = cost;
                 bm.UB = UB; bm.Bc = Bc; bm.nub = nub; bm.nbg = nbg; bm.ctas = ctas; bm.NH = NH; bm.R = 8;
                 bm.smem_fwd = sf; bm.smem_bwd = sb;
-                bm.mma = (g_lstm_mode != 2 && (H / 32) % 2 == 0) ? 2 : 1;   // 2: twelve accumulator chains per warp
+                bm.mma = ((H / 32) % 2 == 0) ? 2 : 1;   // 2: twelve accumulator chains per warp
             }
         }
         if (best_mma >= 0 && (best_cost < 0 || 2 * best_mma <= 3 * best_cost)) {
@@ -1453,11 +1405,12 @@ struct LstmVariant {
     int gen;      // 1: wgmma (lstm_umma.cu), 2: 3xTF32 mma.sync, 3: packed fp32 FMA
     int UB;       // unit block
     int UBP;      // template unit block: the wgmma forward's UB rounded up to 8 / 12 / 16; UB elsewhere
-    int poll;     // exchange protocol of the wgmma kernels: 1 = data-is-the-flag polling, 0 = flag + bulk copy
-    int strict;   // 1: formal acquire after the flag poll (wgmma flag protocol under debug mode 256)
+    int poll;     // exchange protocol of the wgmma kernels: 1 = data-is-the-flag polling (backward), 0 = flag + bulk
+                  // copy (forward)
+    int strict;   // 1: formal acquire after the flag poll (wgmma forward under debug mode 256)
     int nsplit;   // consecutive launches over row blocks
-    int form;     // mma.sync forward: 0 = fwd_group_mma_v2, 1 / 2 = fwd_group_mma<1> / <2>;
-                  // mma.sync backward: 0 = one polling warp per group, 1 = every warp polls (flag bit 2); FMA: NH
+    int form;     // mma.sync forward: 0 = fwd_group_mma_v2, 1 / 2 = fwd_group_mma<1> / <2>; mma.sync backward: 0;
+                  // FMA: NH
     int R;        // FMA register tile rows (4 or 8)
     int vec;      // 1: the UB % 4 == 0 store path (wgmma forward publish, FMA backward scatter), 0: scalar stores
 };
@@ -1466,27 +1419,23 @@ static int lstm_variant(int B, int H, int ndir, bool bwd, Plan* pl, LstmVariant*
     const int rc = make_plan(B, H, ndir, pl);
     if (rc != 0) return rc;
     *v = LstmVariant{};
-    const int uf = g_lstm_flags >> 4;
-    if (!bwd && g_lstm_mode == 0 && lstm_umma_fwd_variant(B, H, ndir, uf, &v->UB, &v->UBP, &v->poll, &v->nsplit)) {
+    if (!bwd && g_lstm_mode == 0 && lstm_umma_fwd_variant(B, H, ndir, &v->UB, &v->UBP, &v->nsplit)) {
         v->gen = 1;
-        v->strict = (!v->poll && (uf & 1)) ? 1 : 0;
+        v->strict = g_lstm_strict ? 1 : 0;
         v->vec = (v->UB % 4 == 0) ? 1 : 0;
         return 0;
     }
-    // flag bit 5 (mode 512) toggles the backward between the wgmma kernel and the mma.sync generation
-    if (bwd && g_lstm_mode == 0 && (((g_lstm_flags & 32) != 0) != (LSTM_UMMA_BWD_DEFAULT != 0)) &&
-        lstm_umma_bwd_variant(B, H, ndir, uf, &v->UB, &v->poll, &v->nsplit)) {
+    if (bwd && g_lstm_mode == 0 && lstm_umma_bwd_variant(B, H, ndir, &v->UB, &v->nsplit)) {
         v->gen = 1;
         v->UBP = v->UB;
-        v->strict = (!v->poll && (uf & 1)) ? 1 : 0;
+        v->poll = 1;
         return 0;
     }
     v->UB = v->UBP = pl->UB;
     v->nsplit = pl->nsplit;
     if (pl->mma) {
         v->gen = 2;
-        if (bwd) v->form = (g_lstm_flags & 4) ? 1 : 0;
-        else v->form = (!(g_lstm_flags & 4) && H % 128 == 0) ? 0 : pl->mma;
+        if (!bwd) v->form = (H % 128 == 0) ? 0 : pl->mma;
     } else {
         v->gen = 3;
         v->form = pl->NH;
@@ -1497,7 +1446,6 @@ static int lstm_variant(int B, int H, int ndir, bool bwd, Plan* pl, LstmVariant*
 }
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-static long long* g_trace = nullptr;   // debug only: set through b200asr_debug_set_lstm_trace
 
 }  // namespace b200asr
 
@@ -1547,11 +1495,10 @@ static int bilstm_run(bool bwd, float* gates, const float* w_hh, float* cstate, 
                  "bilstm: no feasible decomposition for B=%d H=%d ndir=%d (H must be a multiple of 16)", B, H, ndir);
     B200_REQUIRE(workspace_bytes >= b200asr_bilstm_workspace_bytes(B, T, H, ndir), "bilstm: workspace too small");
     if (v.gen == 1 && !bwd)
-        return lstm_umma_fwd(gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes,
-                             (g_lstm_flags & 8) ? nullptr : g_trace, g_lstm_flags >> 4, stream);
+        return lstm_umma_fwd(gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes, v.strict != 0,
+                             stream);
     if (v.gen == 1)
-        return lstm_umma_bwd(gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes,
-                             (g_lstm_flags & 8) ? g_trace : nullptr, g_lstm_flags >> 4, stream);
+        return lstm_umma_bwd(gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes, stream);
     unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
     float* packed = reinterpret_cast<float*>(ws);
     const size_t xoff = align_up(pl.pack_bytes, 256);
@@ -1571,8 +1518,7 @@ static int bilstm_run(bool bwd, float* gates, const float* w_hh, float* cstate, 
     LstmParams p;
     p.gates = gates; p.whh = packed; p.cst = cstate; p.out = out_or_dout; p.xbuf = xbuf; p.counters = counters;
     p.err_flag = err_flag; p.B = B; p.T = T; p.H = H; p.ndir = ndir; p.UB = pl.UB; p.Bc = pl.Bc; p.nub = pl.nub;
-    p.nbg = pl.nbg; p.NH = pl.NH; p.R = pl.R; p.mma = pl.mma; p.form = v.form; p.flags = g_lstm_flags;
-    p.trace = (bwd == ((g_lstm_flags & 8) != 0)) ? g_trace : nullptr;   // flag bit 3: trace the backward kernel
+    p.nbg = pl.nbg; p.NH = pl.NH; p.R = pl.R; p.mma = pl.mma; p.form = v.form;
     const void* fn = !pl.mma ? (bwd ? (const void*)bilstm_bwd_kernel : (const void*)bilstm_fwd_kernel)
                              : (bwd ? (const void*)bilstm_bwd_mma_kernel : (const void*)bilstm_fwd_mma_kernel);
     const size_t smem = bwd ? pl.smem_bwd : pl.smem_fwd;
@@ -1604,10 +1550,9 @@ extern "C" int b200asr_debug_lstm_variant(int B, int H, int ndir, int bwd, int* 
     return 0;
 }
 
-extern "C" void b200asr_debug_set_lstm_trace(long long* device_buffer) { g_trace = device_buffer; }
 extern "C" void b200asr_debug_set_lstm_mode(int mode) {
     g_lstm_mode = mode & 3;
-    g_lstm_flags = mode >> 4;
+    g_lstm_strict = (mode & 256) != 0;
 }
 
 extern "C" int b200asr_bilstm_fwd(float* gates, const float* w_hh, float* cstate, float* out, int B, int T, int H,

@@ -48,8 +48,8 @@ struct UlParams {
     uint8_t* xbuf;         // [ndir][nbg][2] images of the A operand
     unsigned* counters;    // [ndir][nbg]
     int* err_flag;
-    long long* trace;
-    int B, T, H, ndir, UB, nub, nbg, NA, NC, flags;
+    int B, T, H, ndir, UB, nub, nbg, NA, NC;
+    int strict;            // forward: formal acquire after the flag poll (debug mode 256)
     int b0, Bend;
 };
 
@@ -81,26 +81,7 @@ __device__ __forceinline__ void ul_spin_until(const unsigned* ctr, unsigned targ
         fence_proxy_async();
     }
 }
-// ---- "data is the flag" exchange (UL_POLL kernels) ----------------------------------------------------------------
-// The exchange buffers start out filled with a bit pattern that a real value never takes (fp16 0xFFFF / fp32
-// 0xFFFFFFFF: NaNs that arithmetic does not produce).  A producer just STORES its slice; a consumer polls the data with
-// relaxed gpu-scope loads (served at L2) until no poison is left, so a step's hand-over costs one store -> L2 -> load
-// round trip instead of  fence -> flag -> poll -> bulk copy.  Buffers rotate over UL_NBUF steps; the producer re-poisons
-// its slice of the buffer that will be written again UL_NBUF-2 steps later - at that point every consumer is provably
-// done with it (they all published the step after reading it).
-constexpr int UL_NBUF = 8;
-#ifndef UL_POLL_FWD_DEFAULT
-#define UL_POLL_FWD_DEFAULT 0     // 1 once the polling exchange of the forward kernel is the validated default
-#endif
-#ifndef UL_POLL_BWD_DEFAULT
-#define UL_POLL_BWD_DEFAULT 1
-#endif
-__device__ __forceinline__ uint4 ld_relaxed_v4(const void* p) {
-    uint4 v;
-    asm volatile("ld.relaxed.gpu.global.v4.u32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-    return v;
-}
+// ---- the backward's "data is the flag" exchange: relaxed gpu-scope loads and stores of tagged partials -------------
 __device__ __forceinline__ float ld_relaxed_f32(const float* p) {
     float v;
     asm volatile("ld.relaxed.gpu.global.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
@@ -108,14 +89,6 @@ __device__ __forceinline__ float ld_relaxed_f32(const float* p) {
 }
 __device__ __forceinline__ void st_relaxed_v2(void* p, uint32_t a, uint32_t b) {
     asm volatile("st.relaxed.gpu.global.v2.u32 [%0], {%1,%2};" ::"l"(p), "r"(a), "r"(b) : "memory");
-}
-__device__ __forceinline__ void st_relaxed_b16(void* p, unsigned short a) {
-    asm volatile("st.relaxed.gpu.global.u16 [%0], %1;" ::"l"(p), "h"(a) : "memory");
-}
-// any 16-bit half of the chunk still 0xFFFF?
-__device__ __forceinline__ bool has_poison16(const uint4& v) {
-    return (__vcmpeq2(v.x, 0xFFFFFFFFu) | __vcmpeq2(v.y, 0xFFFFFFFFu) | __vcmpeq2(v.z, 0xFFFFFFFFu) |
-            __vcmpeq2(v.w, 0xFFFFFFFFu)) != 0u;
 }
 __device__ __forceinline__ void ul_watchdog(long long t0, int* err_flag) {
     if (clock64() - t0 > (1LL << 33)) {  // ~4 s: a peer died; abort instead of hanging the GPU
@@ -162,14 +135,11 @@ __global__ void ul_pack_fwd_kernel(const float* __restrict__ w, uint8_t* __restr
     }
 }
 
-#define UL_TRACE(slot) \
-    do { if (p.trace && blockIdx.x == 0) p.trace[(size_t)step * 16 + (slot)] = clock64(); } while (0)
-
 // Warp roles: warps [0, UBP) MMA + epilogue / pointwise - UBP/4 warpgroups; warp w is warp q = w % 4 of warpgroup
 // j = w / 4 (the unit quad), i.e. ONE cell (batch row 8q + lane/4, unit 4j + lane%4) per thread; warp UBP = publisher
 // (one lane: ONE gpu-scope fence + release per CTA and step, after the epilogue warps arrived on `pub`); warps
 // UBP+1 .. UBP+NC = control, one lane each, control warp c owns K atoms c, c+NC, ...
-template <int UBP, bool POLL>
+template <int UBP>
 __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_umma_kernel(UlParams p) {
     constexpr int N = 8 * UBP;            // B operand rows (gate columns, hi + lo copies)
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -180,7 +150,6 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
     uint64_t* mma_done = full + UL_MAX_ATOMS;    // the MMAs of a step have read every atom of A (one arrival per warp)
     uint64_t* wload = mma_done + 1;
     uint64_t* pub = mma_done + 2;                // the epilogue warps have stored h_step
-    uint64_t* landed = mma_done + 3;             // [UL_MAX_ATOMS] polling exchange: a bulk copy of the atom has landed
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int NC = p.NC;
@@ -190,10 +159,7 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
     const int dir = blk;
 
     if (tid == 0) {
-        for (int a = 0; a < UL_MAX_ATOMS; ++a) {
-            mbar_init(&full[a], 1);
-            mbar_init(&landed[a], 1);
-        }
+        for (int a = 0; a < UL_MAX_ATOMS; ++a) mbar_init(&full[a], 1);
         mbar_init(pub, UBP);
         mbar_init(mma_done, UBP);
         mbar_init(wload, 1);
@@ -201,77 +167,18 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
     }
     __syncthreads();
     const size_t img_bytes = (size_t)NA * UL_ATOM_A;             // one image of the A operand
-    uint8_t* xb = p.xbuf + ((size_t)dir * p.nbg + bg) * (POLL ? UL_NBUF : 2) * img_bytes;
+    uint8_t* xb = p.xbuf + ((size_t)dir * p.nbg + bg) * 2 * img_bytes;
     unsigned* ctr0 = p.counters + ((size_t)dir * p.nbg + bg) * UL_MAX_ATOMS;
 
-    if (POLL && warp >= UBP) {
-        // ------------------------------------------------------------------ loader warps (warp UBP only loads W)
-        const int c = warp - UBP;                     // 0 .. UL_MAX_CTRL
-        if (c == 0) {
-            if (lane == 0) {
-                const uint8_t* wsrc = p.wpack + ((size_t)dir * p.nub + ub) * ((size_t)NA * N * 128);
-                mbar_expect_tx(wload, (uint32_t)(NA * N * 128));
-                for (int a = 0; a < NA; ++a)
-                    bulk_g2s(sB + (size_t)a * N * 128, wsrc + (size_t)a * N * 128, N * 128, wload);
-            }
-        } else {
-            // loader warp c-1 owns K atoms c-1, c-1+NC, ...  Per atom and step: (1) lanes 0..7 spin on the LAST row of the
-            // atom in the exchange buffer (8 chunks = a slice of every producer) until no poison is left - the data
-            // itself is the flag, nobody fences; (2) lane 0 pulls the atom with ONE bulk copy; (3) the warp checks the
-            // landed image for poison (a slower producer warp's rows may lag the sentinel row) and re-pulls if needed;
-            // (4) the atom is released to the MMA lane.
-            uint32_t nland[2] = {0u, 0u};                 // bulk copies completed per owned atom (barrier phase)
-            for (int step = 0; step + 1 < T; ++step) {
-                // my own MMAs of `step` (which read the atoms about to be overwritten) are done
-                if (step > 0) mbar_wait(mma_done, (uint32_t)((step - 1) & 1));
-                const uint8_t* img = xb + (size_t)(step % UL_NBUF) * img_bytes;
-                int own = 0;
-                for (int a = c - 1; a < NA; a += NC, ++own) {
-                    const uint8_t* src = img + (size_t)a * UL_ATOM_A;
-                    uint8_t* dst = sA + (size_t)a * UL_ATOM_A;
-                    const long long t0 = clock64();
-                    bool bad = true;
-                    while (bad) {
-                        if (lane < 8) {
-                            uint4 v = ld_relaxed_v4(src + 63 * 128 + lane * 16);
-                            while (has_poison16(v)) {
-                                ul_watchdog(t0, p.err_flag);
-                                v = ld_relaxed_v4(src + 63 * 128 + lane * 16);
-                            }
-                        }
-                        __syncwarp();
-                        if (a == 0 && lane == 0) UL_TRACE(10);
-                        if (lane == 0) {
-                            mbar_expect_tx(&landed[a], UL_ATOM_A);
-                            bulk_g2s(dst, src, UL_ATOM_A, &landed[a]);
-                        }
-                        mbar_wait(&landed[a], nland[own & 1] & 1u);
-                        ++nland[own & 1];
-                        bool p16 = false;
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            p16 |= has_poison16(*reinterpret_cast<const uint4*>(dst + (size_t)(j * 32 + lane) * 16));
-                        bad = __any_sync(0xffffffffu, p16);
-                        if (bad) ul_watchdog(t0, p.err_flag);
-                    }
-                    __syncwarp();
-                    if (lane == 0) ul_arrive(&full[a]);
-                    if (a == 0 && lane == 0) UL_TRACE(11);
-                    if (a == NA - 1 && lane == 0) UL_TRACE(15);
-                }
-            }
-        }
-    } else if (warp == UBP) {
+    if (warp == UBP) {
         // ------------------------------------------------------------------ publisher lane
         if (lane == 0) {
             const int a0 = (ub * UB) >> 6, a1 = (ub * UB + UB - 1) >> 6;
             for (int step = 0; step + 1 < T; ++step) {
                 mbar_wait(pub, (uint32_t)(step & 1));       // every epilogue warp stored its part of h_step
-                UL_TRACE(8);
                 fence_acq_rel_gpu();                        // their stores (observed through the mbarrier) first ...
                 red_relaxed_add_u32(ctr0 + a0, 1u);         // ... then the flag(s) of the K atom(s) of my unit block
                 if (a1 != a0) red_relaxed_add_u32(ctr0 + a1, 1u);
-                UL_TRACE(9);
             }
         }
     } else if (warp > UBP) {
@@ -296,13 +203,10 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
                 // ago: every producer ran the same MMAs before it could publish)
                 if (step > 0) mbar_wait(mma_done, (uint32_t)((step - 1) & 1));
                 for (int i = 0, a = c; a < NA; a += NC, ++i) {
-                    ul_spin_until(ctr0 + a, (unsigned)(step + 1) * per_step[i], p.err_flag, (p.flags & 1) != 0);
-                    if (a == 0) UL_TRACE(10);
-                    if (a == NA - 1) UL_TRACE(15);
+                    ul_spin_until(ctr0 + a, (unsigned)(step + 1) * per_step[i], p.err_flag, p.strict != 0);
                     const uint8_t* src = xb + (size_t)(step & 1) * ((size_t)NA * UL_ATOM_A) + (size_t)a * UL_ATOM_A;
                     mbar_expect_tx(&full[a], UL_ATOM_A);
                     bulk_g2s(sA + (size_t)a * UL_ATOM_A, src, UL_ATOM_A, &full[a]);
-                    if (a == 0) UL_TRACE(11);
                 }
             }
         }
@@ -319,7 +223,6 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
         const uint32_t pub_hi = (uint32_t)(ug >> 6) * UL_ATOM_A + wgmma::sw128_offset(a_row_hi, (ug & 63) * 2);
         const uint32_t pub_lo = (uint32_t)(ug >> 6) * UL_ATOM_A + wgmma::sw128_offset(a_row_lo, (ug & 63) * 2);
         float c_reg = 0.f;
-        const bool trc = (warp == 0 && lane == 0);
         float4 st_g = make_float4(0.f, 0.f, 0.f, 0.f);
         float st_c = 0.f, st_h = 0.f;
         size_t st_row = 0, st_out = 0;
@@ -327,7 +230,6 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
 
         for (int step = 0; step < T; ++step) {
             const int tt = dir ? (T - 1 - step) : step;
-            if (trc) UL_TRACE(0);
             const size_t rowbase = ((size_t)dir * p.B + (ok ? brow : 0)) * T + tt;
             float4 pre = make_float4(0.f, 0.f, 0.f, 0.f);
             if (ok) pre = *reinterpret_cast<const float4*>(p.gates + (rowbase * H + ug) * 4);
@@ -337,23 +239,18 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
                 wgmma::fence();
                 for (int a = 0; a < NA; ++a) {
                     mbar_wait(&full[a], (uint32_t)((step - 1) & 1));
-                    if (trc && a == 0) UL_TRACE(1);
-                    if (trc && a == NA - 1) UL_TRACE(6);
 #pragma unroll
                     for (int j = 0; j < 4; ++j)
                         wgmma::mma_f16_n32(d, wgmma::desc_k_sw128(a_base + a * UL_ATOM_A + j * 32),
                                            wgmma::desc_k_sw128(b_base + a * (N * 128) + j * 32), (a | j) != 0);
                 }
                 wgmma::commit_group();
-                if (trc) UL_TRACE(2);
                 wgmma::wait_all();
                 wgmma::fence_operand(d);
                 __syncwarp();
                 if (lane == 0) ul_arrive(mma_done);     // the control warps may overwrite the atoms of A
-                if (trc) UL_TRACE(3);
                 // d[0..7]: hi and lo row against W_hi, gates (i,f) then (g,o); d[8..15]: the same against W_lo
                 const float *dif = d, *dgo = d + 4, *eif = d + 8, *ego = d + 12;
-                if (trc) UL_TRACE(4);
                 if (st_pending) {
                     *reinterpret_cast<float4*>(p.gates + (st_row * H + ug) * 4) = st_g;
                     p.cst[st_row * H + ug] = st_c;
@@ -373,58 +270,29 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
             const float c = fmaf(fg, c_reg, ig * gg);
             c_reg = ok ? c : 0.f;
             const float hq = ok ? og * tanhf(c) : 0.f;
-            if (trc) UL_TRACE(7);
             if (step + 1 < T) {
                 // publish h_step as element (A row, k = ug) of the next A operand, fp16 hi / lo
-                uint8_t* dstimg = xb + (size_t)(POLL ? (step % UL_NBUF) : (step & 1)) * img_bytes;
-                if (POLL) {
-                    // data is the flag: plain gpu-scope stores; re-poison my slice of the buffer used UL_NBUF-2 steps on
-                    uint8_t* poison = xb + (size_t)((step + UL_NBUF - 2) % UL_NBUF) * img_bytes;
-                    __half hi, lo;
-                    split_f16(hq, hi, lo);
-                    if ((UB & 3) == 0) {
-                        uint32_t wh = __half_as_ushort(hi), wl = __half_as_ushort(lo);
-                        wh |= __shfl_down_sync(0xffffffffu, wh, 1) << 16;
-                        wl |= __shfl_down_sync(0xffffffffu, wl, 1) << 16;
-                        const uint32_t wh2 = __shfl_down_sync(0xffffffffu, wh, 2);
-                        const uint32_t wl2 = __shfl_down_sync(0xffffffffu, wl, 2);
-                        if (tq == 0 && unit < UB) {
-                            st_relaxed_v2(poison + pub_hi, 0xFFFFFFFFu, 0xFFFFFFFFu);
-                            st_relaxed_v2(poison + pub_lo, 0xFFFFFFFFu, 0xFFFFFFFFu);
-                            st_relaxed_v2(dstimg + pub_hi, wh, wh2);
-                            st_relaxed_v2(dstimg + pub_lo, wl, wl2);
-                        }
-                    } else if (unit < UB) {
-                        st_relaxed_b16(poison + pub_hi, 0xFFFFu);
-                        st_relaxed_b16(poison + pub_lo, 0xFFFFu);
-                        st_relaxed_b16(dstimg + pub_hi, __half_as_ushort(hi));
-                        st_relaxed_b16(dstimg + pub_lo, __half_as_ushort(lo));
+                uint8_t* dstimg = xb + (size_t)(step & 1) * img_bytes;
+                __half hi, lo;
+                split_f16(hq, hi, lo);
+                if ((UB & 3) == 0) {
+                    // the four lanes of a unit quad hold k = ug .. ug+3 of the same A row: one 8-byte store each
+                    // for the hi and the lo row instead of four 2-byte ones
+                    uint32_t wh = __half_as_ushort(hi), wl = __half_as_ushort(lo);
+                    wh |= __shfl_down_sync(0xffffffffu, wh, 1) << 16;
+                    wl |= __shfl_down_sync(0xffffffffu, wl, 1) << 16;
+                    const uint32_t wh2 = __shfl_down_sync(0xffffffffu, wh, 2);
+                    const uint32_t wl2 = __shfl_down_sync(0xffffffffu, wl, 2);
+                    if (tq == 0 && unit < UB) {
+                        *reinterpret_cast<uint2*>(dstimg + pub_hi) = make_uint2(wh, wh2);
+                        *reinterpret_cast<uint2*>(dstimg + pub_lo) = make_uint2(wl, wl2);
                     }
-                } else {
-                    __half hi, lo;
-                    split_f16(hq, hi, lo);
-                    if ((UB & 3) == 0) {
-                        // the four lanes of a unit quad hold k = ug .. ug+3 of the same A row: one 8-byte store each
-                        // for the hi and the lo row instead of four 2-byte ones
-                        uint32_t wh = __half_as_ushort(hi), wl = __half_as_ushort(lo);
-                        wh |= __shfl_down_sync(0xffffffffu, wh, 1) << 16;
-                        wl |= __shfl_down_sync(0xffffffffu, wl, 1) << 16;
-                        const uint32_t wh2 = __shfl_down_sync(0xffffffffu, wh, 2);
-                        const uint32_t wl2 = __shfl_down_sync(0xffffffffu, wl, 2);
-                        if (tq == 0 && unit < UB) {
-                            *reinterpret_cast<uint2*>(dstimg + pub_hi) = make_uint2(wh, wh2);
-                            *reinterpret_cast<uint2*>(dstimg + pub_lo) = make_uint2(wl, wl2);
-                        }
-                    } else if (unit < UB) {
-                        *reinterpret_cast<__half*>(dstimg + pub_hi) = hi;
-                        *reinterpret_cast<__half*>(dstimg + pub_lo) = lo;
-                    }
+                } else if (unit < UB) {
+                    *reinterpret_cast<__half*>(dstimg + pub_hi) = hi;
+                    *reinterpret_cast<__half*>(dstimg + pub_lo) = lo;
                 }
-                if (!POLL) {
-                    __syncwarp();
-                    if (lane == 0) ul_arrive(pub);
-                }
-                if (trc) UL_TRACE(5);
+                __syncwarp();
+                if (lane == 0) ul_arrive(pub);
             }
             // the stash / output stores of this step are issued during the NEXT step (after its MMAs): stores
             // in flight while the publisher runs its gpu-scope fence lengthen that fence by their L2 round trip
@@ -488,12 +356,14 @@ __device__ __forceinline__ float add_ftz(float a, float b) {
 constexpr int ULB_EPI_WARPS = 16;
 constexpr int ULB_CTRL = 4;
 
-// POLL = the "data is the flag" exchange for the backward: every fp32 partial carries the parity of its buffer
-// generation in its least significant mantissa bit (2^-24 relative - below the resolution of the hi/lo product), the
-// destination polls its inbox IN GLOBAL MEMORY (L2) with relaxed loads until every word shows the expected tag and sums
-// straight from registers (flushing subnormals, so that a tagged zero adds nothing): no fence, no counter, no bulk
-// copy, no shared-memory inbox.
-template <int UB, bool POLL>
+// The state exchange is "data is the flag": every fp32 partial carries the parity of its buffer generation in its
+// least significant mantissa bit (2^-24 relative - below the resolution of the hi/lo product), the destination polls
+// its inbox IN GLOBAL MEMORY (L2) with relaxed loads until every word shows the expected tag and sums straight from
+// registers (flushing subnormals, so that a tagged zero adds nothing): no fence, no counter, no bulk copy, no
+// shared-memory inbox.
+// Warp roles: warps [0, 16) pointwise + MMA + drain; lane 0 of warp 17 loads W_hh.  Warps 16 and 18 .. 20 have no work
+// but stay in the block: __launch_bounds__ and ul_launch_bwd's occupancy check count them.
+template <int UB>
 __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm_bwd_umma_kernel(UlParams p) {
     constexpr int KS = (4 * UB) / 16;               // MMAs (k-steps of 16) per product and n-block
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -503,14 +373,10 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
     uint8_t* sWlo = smem + (size_t)H * 128;
     uint8_t* sA1 = sWlo + (size_t)H * 128;
     uint8_t* sA2 = sA1 + 8192;
-    float* inbox = reinterpret_cast<float*>(sA2 + 8192);                       // [nub][32][UB]
-    const size_t inbox_bytes = POLL ? 0 : (size_t)nub * UL_BC * UB * sizeof(float);   // POLL sums straight from L2
-    float* rscale = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(inbox) + inbox_bytes);   // [32]
-    uint64_t* in_full = reinterpret_cast<uint64_t*>(rscale + 32);
-    uint64_t* a_ready = in_full + 1;
-    uint64_t* mma_done = in_full + 2;               // the MMAs of a step have read the A tiles (one arrival per warp)
-    uint64_t* pub = in_full + 3;
-    uint64_t* wload = in_full + 4;
+    float* rscale = reinterpret_cast<float*>(sA2 + 8192);                      // [32]
+    uint64_t* a_ready = reinterpret_cast<uint64_t*>(rscale + 32);
+    uint64_t* mma_done = a_ready + 1;               // the MMAs of a step have read the A tiles (one arrival per warp)
+    uint64_t* wload = a_ready + 2;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     int blk = blockIdx.x;
@@ -520,10 +386,8 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
 
     for (int i = tid; i < 16384 / 16; i += blockDim.x) reinterpret_cast<uint4*>(sA1)[i] = make_uint4(0, 0, 0, 0);
     if (tid == 0) {
-        mbar_init(in_full, ULB_CTRL);
         mbar_init(a_ready, ULB_EPI_WARPS);
         mbar_init(mma_done, ULB_EPI_WARPS);
-        mbar_init(pub, ULB_EPI_WARPS);
         mbar_init(wload, 1);
         mbar_fence_init();
     }
@@ -531,48 +395,13 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
     __syncthreads();
     const size_t xelems = (size_t)nub * nub * UL_BC * UB;                       // one parity buffer of one (dir, bg)
     float* xb = reinterpret_cast<float*>(p.xbuf) + ((size_t)dir * p.nbg + bg) * 2 * xelems;
-    unsigned* ctr = p.counters + ((size_t)dir * p.nbg + bg);
 
-    if (POLL && warp >= ULB_EPI_WARPS) {
-        if (warp == ULB_EPI_WARPS + 1 && lane == 0) {            // only the W load is left for the control warps
+    if (warp >= ULB_EPI_WARPS) {
+        if (warp == ULB_EPI_WARPS + 1 && lane == 0) {
             const uint8_t* wsrc = p.wpack + ((size_t)dir * p.nub + ub) * ((size_t)2 * H * 128);
             mbar_expect_tx(wload, (uint32_t)(2 * H * 128));
             for (int off = 0; off < 2 * H * 128; off += 32768)
                 bulk_g2s(sWhi + off, wsrc + off, 32768, wload);
-        }
-    } else if (warp == ULB_EPI_WARPS) {
-        // ------------------------------------------------------------------ publisher lane
-        if (lane == 0) {
-            for (int step = 0; step + 1 < T; ++step) {
-                mbar_wait(pub, (uint32_t)(step & 1));
-                UL_TRACE(8);
-                fence_acq_rel_gpu();
-                red_relaxed_add_u32(ctr, 1u);
-                UL_TRACE(9);
-            }
-        }
-    } else if (warp > ULB_EPI_WARPS) {
-        // ------------------------------------------------------------------ control lanes: W load, inbox pulls
-        const int c = warp - ULB_EPI_WARPS - 1;
-        if (lane == 0) {
-            if (c == 0) {
-                const uint8_t* wsrc = p.wpack + ((size_t)dir * p.nub + ub) * ((size_t)2 * H * 128);
-                mbar_expect_tx(wload, (uint32_t)(2 * H * 128));
-                for (int off = 0; off < 2 * H * 128; off += 32768)
-                    bulk_g2s(sWhi + off, wsrc + off, 32768, wload);
-            }
-            const uint32_t chunk = (uint32_t)(inbox_bytes / ULB_CTRL);
-            for (int step = 0; step + 1 < T; ++step) {
-                // my epilogue warps summed the inbox of `step` before they released the A tile of `step`
-                mbar_wait(mma_done, (uint32_t)(step & 1));
-                ul_spin_until(ctr, (unsigned)(step + 1) * (unsigned)nub, p.err_flag, (p.flags & 1) != 0);
-                if (c == 0) UL_TRACE(10);
-                const uint8_t* src = reinterpret_cast<const uint8_t*>(xb + (size_t)(step & 1) * xelems +
-                                                                      (size_t)ub * nub * UL_BC * UB) + (size_t)c * chunk;
-                mbar_expect_tx(in_full, chunk);
-                bulk_g2s(reinterpret_cast<uint8_t*>(inbox) + (size_t)c * chunk, src, chunk, in_full);
-                if (c == 0) UL_TRACE(11);
-            }
         }
     } else {
         // ------------------------------------------------------------------ pointwise + MMA + drain warps
@@ -591,13 +420,11 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
         const uint32_t a1 = smem_u32(sA1), a2 = smem_u32(sA2), whi = smem_u32(sWhi), wlo = smem_u32(sWlo);
         float d[32];
         float dc_reg = 0.f;
-        const bool trc = (warp == 0 && lane == 0);
 
         for (int step = 0; step < T; ++step) {
             const int fstep = T - 1 - step;
             const int tt = dir ? (T - 1 - fstep) : fstep;
             const int tt_prev = dir ? tt + 1 : tt - 1;
-            if (trc) UL_TRACE(0);
             float4 gtv = make_float4(0.f, 0.f, 0.f, 0.f);
             float ct = 0.f, cp = 0.f, dh = 0.f;
             const size_t row = ((size_t)dir * p.B + (ok ? brow : 0)) * T + tt;
@@ -607,7 +434,7 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
                 if (fstep > 0) cp = p.cst[(((size_t)dir * p.B + brow) * T + tt_prev) * H + ug];
                 dh = p.out[((size_t)brow * T + tt) * (p.ndir * H) + (size_t)dir * H + ug];
             }
-            if (POLL && step > 0) {
+            if (step > 0) {
                 if (cell) {
                     const float* ib = xb + (size_t)((step - 1) & 1) * xelems + (size_t)ub * nub * UL_BC * UB +
                                       (size_t)b * UB + u;                       // [src] stride UL_BC * UB
@@ -650,24 +477,6 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
                     }
                     dh += (s0 + s1) + (s2 + s3);
                 }
-                if (trc) UL_TRACE(3);
-            }
-            if (!POLL && step > 0) {
-                mbar_wait(in_full, (uint32_t)((step - 1) & 1));
-                if (trc) UL_TRACE(3);
-                if (cell) {
-                    const float* ib = inbox + (size_t)b * UB + u;
-                    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-                    int s = 0;
-                    for (; s + 3 < nub; s += 4) {
-                        s0 += ib[(size_t)s * UL_BC * UB];
-                        s1 += ib[(size_t)(s + 1) * UL_BC * UB];
-                        s2 += ib[(size_t)(s + 2) * UL_BC * UB];
-                        s3 += ib[(size_t)(s + 3) * UL_BC * UB];
-                    }
-                    for (; s < nub; ++s) s0 += ib[(size_t)s * UL_BC * UB];
-                    dh += (s0 + s1) + (s2 + s3);
-                }
             }
             float4 dg = make_float4(0.f, 0.f, 0.f, 0.f);
             if (ok) {
@@ -681,7 +490,6 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
                 dc_reg = dc * fg;
                 *reinterpret_cast<float4*>(p.gates + (row * H + ug) * 4) = dg;
             }
-            if (trc) UL_TRACE(4);
             if (step + 1 < T) {
                 // per-row power-of-two scale: the row's largest |dG| goes to [2^13, 2^14)
                 float m = fmaxf(fmaxf(fabsf(dg.x), fabsf(dg.y)), fmaxf(fabsf(dg.z), fabsf(dg.w)));
@@ -712,10 +520,8 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
                 fence_proxy_async_smem();       // my generic-proxy writes of the A tiles -> visible to the tensor core
                 __syncwarp();
                 if (lane == 0) ul_arrive(a_ready);
-                if (trc) UL_TRACE(5);
                 if (step == 0) mbar_wait(wload, 0);
                 mbar_wait(a_ready, (uint32_t)(step & 1));           // all 16 warps wrote (and fenced) their part of A
-                if (trc) UL_TRACE(1);
                 // ---- MMA + drain of the accumulator into the destinations' inboxes, n-block by n-block
                 float* outbase = xb + (size_t)(step & 1) * xelems;
                 for (int j = 0; j < NB; ++j) {
@@ -731,7 +537,6 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
                     wgmma::commit_group();
                     wgmma::wait_all();
                     wgmma::fence_operand(d);
-                    if (trc && j == 0) UL_TRACE(6);
                     const float* v0 = d;
                     const float* v1 = d + 16;
                     const float rs = rscale[drow];
@@ -746,21 +551,13 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
                             const float o0 = (v[0] + v[2] * k) * rs;
                             const float o1 = (v[1] + v[3] * k) * rs;
                             float* optr = outbase + (((size_t)dst * nub + ub) * UL_BC + drow) * UB + uu;
-                            if (POLL) {
-                                const uint32_t tagw = (uint32_t)((step >> 1) & 1) ^ 1u;
-                                st_relaxed_v2(optr, (__float_as_uint(o0) & ~1u) | tagw, (__float_as_uint(o1) & ~1u) | tagw);
-                            } else {
-                                *reinterpret_cast<float2*>(optr) = make_float2(o0, o1);
-                            }
+                            const uint32_t tagw = (uint32_t)((step >> 1) & 1) ^ 1u;
+                            st_relaxed_v2(optr, (__float_as_uint(o0) & ~1u) | tagw, (__float_as_uint(o1) & ~1u) | tagw);
                         }
                     }
                 }
                 __syncwarp();
-                if (lane == 0) {
-                    ul_arrive(mma_done);
-                    if (!POLL) ul_arrive(pub);
-                }
-                if (trc) UL_TRACE(7);
+                if (lane == 0) ul_arrive(mma_done);
             }
         }
     }
@@ -792,7 +589,7 @@ int ul_plan(int B, int H, int ndir, UlPlan* out) {
             out->UB = UB; out->UBp = UBp; out->nub = nub; out->nbg = nbg; out->ctas = ctas; out->NA = NA;
             out->Bsub = Bs; out->nsplit = (B + Bs - 1) / Bs; out->smem = smem;
             out->pack_bytes = (size_t)ndir * nub * NA * 8 * UBp * 128;
-            out->xbuf_bytes = (size_t)ndir * nbg * UL_NBUF * NA * UL_ATOM_A;   // (2 images suffice for the flag protocol)
+            out->xbuf_bytes = (size_t)ndir * nbg * 2 * NA * UL_ATOM_A;
             return 0;
         }
         if (Bs <= UL_BC) break;
@@ -802,7 +599,7 @@ int ul_plan(int B, int H, int ndir, UlPlan* out) {
 
 size_t ul_align(size_t x) { return (x + 255) / 256 * 256; }
 
-template <int UBP, bool POLL>
+template <int UBP>
 int ul_launch_fwd(const UlPlan& pl, UlParams p, const float* w_hh, cudaStream_t stream) {
     {
         const long long n = (long long)p.ndir * pl.nub * 8 * UBP * p.H;
@@ -811,7 +608,7 @@ int ul_launch_fwd(const UlPlan& pl, UlParams p, const float* w_hh, cudaStream_t 
         ul_pack_fwd_kernel<UBP><<<blocks, 256, 0, stream>>>(w_hh, const_cast<uint8_t*>(p.wpack), p.H, pl.UB, p.ndir);
         B200_LAUNCH_CHECK("ul_pack_fwd_kernel");
     }
-    const void* fn = (const void*)bilstm_fwd_umma_kernel<UBP, POLL>;
+    const void* fn = (const void*)bilstm_fwd_umma_kernel<UBP>;
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
     int per_sm = 0;
     const int threads = 32 * (UBP + 1 + p.NC);
@@ -822,7 +619,6 @@ int ul_launch_fwd(const UlPlan& pl, UlParams p, const float* w_hh, cudaStream_t 
         p.b0 = sp * pl.Bsub;
         p.Bend = p.b0 + pl.Bsub < p.B ? p.b0 + pl.Bsub : p.B;
         B200_CUDA(cudaMemsetAsync(p.counters, 0, UL_COUNTER_BYTES, stream));
-        if (POLL) B200_CUDA(cudaMemsetAsync(p.xbuf, 0xFF, pl.xbuf_bytes, stream));      // poison every exchange image
         void* args[] = {&p};
         B200_CUDA(cudaLaunchCooperativeKernel(fn, dim3(pl.ctas), dim3(threads), args, pl.smem, stream));
         count_launch();
@@ -835,7 +631,7 @@ struct UlbPlan {
     size_t smem, pack_bytes, xbuf_bytes;
 };
 
-int ulb_plan(int B, int H, int ndir, bool poll, UlbPlan* out) {
+int ulb_plan(int B, int H, int ndir, UlbPlan* out) {
     // accumulator = H columns in n-blocks of 256, 64 per warpgroup: 256 | 512 | 640 | 768 (a last block of 128 or 256)
     if (H % 128 != 0 || H < 256 || H > 768) return -1;
     const int sms = sm_count();
@@ -849,9 +645,8 @@ int ulb_plan(int B, int H, int ndir, bool poll, UlbPlan* out) {
             const int ctas = ndir * nbg * nub;
             if (ctas > sms) continue;
             if (nub % 4) continue;
-            const size_t inbox = (size_t)nub * UL_BC * UB * 4;
-            // the polling exchange keeps no inbox in shared memory (which is what lets H = 640 fit)
-            const size_t smem = (size_t)2 * H * 128 + 16384 + (poll ? 0 : inbox) + 128 + 128;
+            const size_t inbox = (size_t)nub * UL_BC * UB * 4;      // partials one destination receives per step
+            const size_t smem = (size_t)2 * H * 128 + 16384 + 128 + 128;
             if (smem > cap || (inbox / ULB_CTRL) % 16 || (2 * H * 128) % 32768) continue;
             out->UB = UB; out->nub = nub; out->nbg = nbg; out->ctas = ctas; out->Bsub = Bs;
             out->nsplit = (B + Bs - 1) / Bs; out->smem = smem;
@@ -864,7 +659,7 @@ int ulb_plan(int B, int H, int ndir, bool poll, UlbPlan* out) {
     return -2;
 }
 
-template <int UB, bool POLL>
+template <int UB>
 int ul_launch_bwd(const UlbPlan& pl, UlParams p, const float* w_hh, cudaStream_t stream) {
     {
         const long long n = (long long)p.ndir * pl.nub * 2 * p.H * 64;
@@ -873,7 +668,7 @@ int ul_launch_bwd(const UlbPlan& pl, UlParams p, const float* w_hh, cudaStream_t
         ul_pack_bwd_kernel<UB><<<blocks, 256, 0, stream>>>(w_hh, const_cast<uint8_t*>(p.wpack), p.H, p.ndir);
         B200_LAUNCH_CHECK("ul_pack_bwd_kernel");
     }
-    const void* fn = (const void*)bilstm_bwd_umma_kernel<UB, POLL>;
+    const void* fn = (const void*)bilstm_bwd_umma_kernel<UB>;
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
     int per_sm = 0;
     const int threads = 32 * (ULB_EPI_WARPS + 1 + ULB_CTRL);
@@ -884,7 +679,7 @@ int ul_launch_bwd(const UlbPlan& pl, UlParams p, const float* w_hh, cudaStream_t
         p.b0 = sp * pl.Bsub;
         p.Bend = p.b0 + pl.Bsub < p.B ? p.b0 + pl.Bsub : p.B;
         B200_CUDA(cudaMemsetAsync(p.counters, 0, UL_COUNTER_BYTES, stream));
-        if (POLL) B200_CUDA(cudaMemsetAsync(p.xbuf, 0, pl.xbuf_bytes, stream));     // generation tags start at 0
+        B200_CUDA(cudaMemsetAsync(p.xbuf, 0, pl.xbuf_bytes, stream));     // generation tags start at 0
         void* args[] = {&p};
         B200_CUDA(cudaLaunchCooperativeKernel(fn, dim3(pl.ctas), dim3(threads), args, pl.smem, stream));
         count_launch();
@@ -894,34 +689,27 @@ int ul_launch_bwd(const UlbPlan& pl, UlParams p, const float* w_hh, cudaStream_t
 
 }  // namespace
 
-// flag bit 2 (debug mode 1024) / bit 3 (debug mode 2048) select the OTHER exchange protocol of the forward / backward
-static bool ul_poll(int flags) { return ((flags & 4) != 0) != (UL_POLL_FWD_DEFAULT != 0); }
-static bool ulb_poll(int flags) { return ((flags & 8) != 0) != (UL_POLL_BWD_DEFAULT != 0); }
-
-bool lstm_umma_bwd_variant(int B, int H, int ndir, int flags, int* ub, int* poll, int* nsplit) {
+bool lstm_umma_bwd_variant(int B, int H, int ndir, int* ub, int* nsplit) {
     UlbPlan pl;
-    if (ulb_plan(B, H, ndir, ulb_poll(flags), &pl) != 0) return false;
+    if (ulb_plan(B, H, ndir, &pl) != 0) return false;
     *ub = pl.UB;
-    *poll = ulb_poll(flags) ? 1 : 0;
     *nsplit = pl.nsplit;
     return true;
 }
 
-bool lstm_umma_fwd_variant(int B, int H, int ndir, int flags, int* ub, int* ubp, int* poll, int* nsplit) {
+bool lstm_umma_fwd_variant(int B, int H, int ndir, int* ub, int* ubp, int* nsplit) {
     UlPlan pl;
     if (ul_plan(B, H, ndir, &pl) != 0) return false;
     *ub = pl.UB;
     *ubp = pl.UBp;
-    *poll = ul_poll(flags) ? 1 : 0;
     *nsplit = pl.nsplit;
     return true;
 }
 
 int lstm_umma_bwd(float* gates, const float* w_hh, const float* cstate, const float* dout, int B, int T, int H, int ndir,
-                  void* workspace, size_t workspace_bytes, long long* trace, int flags, cudaStream_t stream) {
+                  void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     UlbPlan pl;
-    const bool poll = ulb_poll(flags);
-    B200_REQUIRE(ulb_plan(B, H, ndir, poll, &pl) == 0, "bilstm(umma bwd): unsupported shape B=%d H=%d ndir=%d", B, H, ndir);
+    B200_REQUIRE(ulb_plan(B, H, ndir, &pl) == 0, "bilstm(umma bwd): unsupported shape B=%d H=%d ndir=%d", B, H, ndir);
     B200_REQUIRE(workspace_bytes >= lstm_umma_workspace_bytes(B, H, ndir), "bilstm(umma bwd): workspace too small");
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     UlParams p;
@@ -930,12 +718,11 @@ int lstm_umma_bwd(float* gates, const float* w_hh, const float* cstate, const fl
     p.xbuf = ws + ul_align(pl.pack_bytes);
     p.counters = reinterpret_cast<unsigned*>(ws + ul_align(pl.pack_bytes) + ul_align(pl.xbuf_bytes));
     p.err_flag = reinterpret_cast<int*>(p.counters + (UL_COUNTER_BYTES / 4 - 4));
-    p.trace = trace;
-    p.flags = flags;
     p.B = B; p.T = T; p.H = H; p.ndir = ndir; p.UB = pl.UB; p.nub = pl.nub; p.nbg = pl.nbg; p.NA = 0; p.NC = ULB_CTRL;
+    p.strict = 0;
     p.b0 = 0; p.Bend = B;
-    if (pl.UB == 16) return poll ? ul_launch_bwd<16, true>(pl, p, w_hh, stream) : ul_launch_bwd<16, false>(pl, p, w_hh, stream);
-    return poll ? ul_launch_bwd<8, true>(pl, p, w_hh, stream) : ul_launch_bwd<8, false>(pl, p, w_hh, stream);
+    if (pl.UB == 16) return ul_launch_bwd<16>(pl, p, w_hh, stream);
+    return ul_launch_bwd<8>(pl, p, w_hh, stream);
 }
 
 size_t lstm_umma_workspace_bytes(int B, int H, int ndir) {
@@ -943,11 +730,7 @@ size_t lstm_umma_workspace_bytes(int B, int H, int ndir) {
     UlbPlan pb;
     size_t f = 0, b = 0;
     if (ul_plan(B, H, ndir, &pl) == 0) f = ul_align(pl.pack_bytes) + ul_align(pl.xbuf_bytes) + UL_COUNTER_BYTES;
-    for (int poll = 0; poll < 2; ++poll)
-        if (ulb_plan(B, H, ndir, poll != 0, &pb) == 0) {
-            const size_t bb = ul_align(pb.pack_bytes) + ul_align(pb.xbuf_bytes) + UL_COUNTER_BYTES;
-            b = bb > b ? bb : b;
-        }
+    if (ulb_plan(B, H, ndir, &pb) == 0) b = ul_align(pb.pack_bytes) + ul_align(pb.xbuf_bytes) + UL_COUNTER_BYTES;
     return f > b ? f : b;
 }
 
@@ -961,7 +744,7 @@ int lstm_umma_plan(int B, int H, int ndir, int* unit_block, int* batch_block, in
 }
 
 int lstm_umma_fwd(float* gates, const float* w_hh, float* cstate, float* out, int B, int T, int H, int ndir,
-                  void* workspace, size_t workspace_bytes, long long* trace, int flags, cudaStream_t stream) {
+                  void* workspace, size_t workspace_bytes, bool strict, cudaStream_t stream) {
     UlPlan pl;
     B200_REQUIRE(ul_plan(B, H, ndir, &pl) == 0, "bilstm(umma): unsupported shape B=%d H=%d ndir=%d", B, H, ndir);
     B200_REQUIRE(workspace_bytes >= lstm_umma_workspace_bytes(B, H, ndir), "bilstm(umma): workspace too small");
@@ -972,16 +755,14 @@ int lstm_umma_fwd(float* gates, const float* w_hh, float* cstate, float* out, in
     p.xbuf = ws + ul_align(pl.pack_bytes);
     p.counters = reinterpret_cast<unsigned*>(ws + ul_align(pl.pack_bytes) + ul_align(pl.xbuf_bytes));
     p.err_flag = reinterpret_cast<int*>(p.counters + (UL_COUNTER_BYTES / 4 - 4));
-    p.trace = trace;
-    p.flags = flags;
     p.B = B; p.T = T; p.H = H; p.ndir = ndir; p.UB = pl.UB; p.nub = pl.nub; p.nbg = pl.nbg; p.NA = pl.NA;
     p.NC = pl.NA < UL_MAX_CTRL ? pl.NA : UL_MAX_CTRL;
+    p.strict = strict ? 1 : 0;
     p.b0 = 0; p.Bend = B;
-    const bool poll = ul_poll(flags);
     switch (pl.UBp) {
-        case 8: return poll ? ul_launch_fwd<8, true>(pl, p, w_hh, stream) : ul_launch_fwd<8, false>(pl, p, w_hh, stream);
-        case 12: return poll ? ul_launch_fwd<12, true>(pl, p, w_hh, stream) : ul_launch_fwd<12, false>(pl, p, w_hh, stream);
-        default: return poll ? ul_launch_fwd<16, true>(pl, p, w_hh, stream) : ul_launch_fwd<16, false>(pl, p, w_hh, stream);
+        case 8: return ul_launch_fwd<8>(pl, p, w_hh, stream);
+        case 12: return ul_launch_fwd<12>(pl, p, w_hh, stream);
+        default: return ul_launch_fwd<16>(pl, p, w_hh, stream);
     }
 }
 

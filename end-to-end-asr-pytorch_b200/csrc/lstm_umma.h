@@ -5,15 +5,16 @@
 
 namespace b200asr {
 
-// The instance lstm_umma_fwd / lstm_umma_bwd launch for these sizes and flags: unit block, template unit block,
-// exchange protocol (1 = data-is-the-flag polling, 0 = flag + bulk copy) and number of launches.  false: no plan.
-bool lstm_umma_fwd_variant(int B, int H, int ndir, int flags, int* ub, int* ubp, int* poll, int* nsplit);
-bool lstm_umma_bwd_variant(int B, int H, int ndir, int flags, int* ub, int* poll, int* nsplit);
+// The instance lstm_umma_fwd / lstm_umma_bwd launch for these sizes: unit block, template unit block and number of
+// launches.  false: no plan.
+bool lstm_umma_fwd_variant(int B, int H, int ndir, int* ub, int* ubp, int* nsplit);
+bool lstm_umma_bwd_variant(int B, int H, int ndir, int* ub, int* nsplit);
 int lstm_umma_bwd(float* gates, const float* w_hh, const float* cstate, const float* dout, int B, int T, int H, int ndir,
-                  void* workspace, size_t workspace_bytes, long long* trace, int flags, cudaStream_t stream);
+                  void* workspace, size_t workspace_bytes, cudaStream_t stream);
 size_t lstm_umma_workspace_bytes(int B, int H, int ndir);
 int lstm_umma_plan(int B, int H, int ndir, int* unit_block, int* batch_block, int* n_ctas);
+// strict: the formal acquire after each flag poll (debug mode 256)
 int lstm_umma_fwd(float* gates, const float* w_hh, float* cstate, float* out, int B, int T, int H, int ndir,
-                  void* workspace, size_t workspace_bytes, long long* trace, int flags, cudaStream_t stream);
+                  void* workspace, size_t workspace_bytes, bool strict, cudaStream_t stream);
 
 }  // namespace b200asr

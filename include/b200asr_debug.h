@@ -1,5 +1,5 @@
 /* Test / measurement switches of libb200asr.so.  NOT part of the drop-in boundary (include/b200asr.h): they exist for
- * tests/ (forcing the fallback kernel generations so that they stay covered) and tools/ (clock64 timelines, A/B timing). */
+ * tests/ (forcing the fallback kernel generations so that they stay covered) and tools/ (A/B timing). */
 #ifndef B200ASR_DEBUG_H
 #define B200ASR_DEBUG_H
 #include "b200asr.h"
@@ -7,21 +7,17 @@
 extern "C" {
 #endif
 
-/* debug: when non-NULL, CTA 0 of the next b200asr_bilstm_fwd (or, with mode flag 128, _bwd) calls records clock64 stamps into [T][16] int64 */
-B200ASR_API void b200asr_debug_set_lstm_trace(long long* device_buffer);
 /* debug/test: 0 (default) = wgmma step GEMMs where the shape allows, else 3xTF32 mma.sync wherever the planner finds
  * a 16-row-tile decomposition, else fp32 FMA; 1 = always the packed-fp32-FMA step kernels; 3 = never wgmma (the
- * mma.sync generation).  All are fp32-class and parity-tested.
- * Upper bits (mode >> 4) are test / measurement switches: 512 = the other backward generation (wgmma <-> mma.sync),
- * 1024 / 2048 = the other state-exchange protocol of the wgmma forward / backward kernel (flag + bulk copy <->
- * data-is-the-flag polling), 128 = trace the backward kernel; see tools/time_lstm.py. */
+ * mma.sync generation); 256 = as 0, with the formal acquire (ld.acquire + proxy fence) after each flag poll of the
+ * wgmma forward.  All are fp32-class and parity-tested. */
 B200ASR_API void b200asr_debug_set_lstm_mode(int mode);
 /* test: the step-kernel variant b200asr_bilstm_fwd (bwd = 0) / _bwd (bwd = 1) runs for these sizes under the current
  * lstm mode on the current device (132 SMs / 232448 B of shared memory without one).  Fills desc[9] =
  * {generation (1 wgmma, 2 mma.sync 3xTF32, 3 fp32 FMA), unit block UB, template unit block (UBP of the wgmma forward,
- *  else UB), exchange protocol (1 data-is-the-flag polling, 0 flag + bulk copy), strict acquire, nsplit (launches),
- *  loop form (mma.sync forward 0 = v2, 1 / 2 = fwd_group_mma<1> / <2>; mma.sync backward 0 = one polling warp, 1 =
- *  every warp polls; FMA: halves NH), FMA register-tile rows R, vectorised UB % 4 == 0 stores}.  Returns 0, or < 0
+ *  else UB), exchange protocol of the wgmma kernels (1 data-is-the-flag polling: the backward, 0 flag + bulk copy: the
+ *  forward), strict acquire, nsplit (launches), loop form (mma.sync forward 0 = v2, 1 / 2 = fwd_group_mma<1> / <2>;
+ *  mma.sync backward 0; FMA: halves NH), FMA register-tile rows R, vectorised UB % 4 == 0 stores}.  Returns 0, or < 0
  * when the shape has no plan.  The dispatcher makes its choice through the same function. */
 B200ASR_API int b200asr_debug_lstm_variant(int B, int H, int ndir, int bwd, int* desc);
 /* test: which alpha/beta lattice kernel b200asr_ctc_fwd_bwd(_logits) runs for a padded target width L_max: 1-4 = the

@@ -12,9 +12,8 @@ import torch
 
 VARIANT_FIELDS = ("gen", "UB", "UBP", "poll", "strict", "nsplit", "form", "R", "vec")
 GEN = {1: "wgmma", 2: "mma.sync", 3: "fma"}
-# debug modes the dispatcher knows (include/b200asr_debug.h): 0 default, 1 FMA only, 3 no wgmma, 256 strict acquire,
-# 512 the other backward generation, 1024 / 2048 the other exchange protocol of the wgmma forward / backward
-SWEEP_MODES = (0, 1, 3, 256, 512, 1024, 2048, 256 + 2048)
+# debug modes the dispatcher knows (include/b200asr_debug.h): 0 default, 1 FMA only, 3 no wgmma, 256 strict acquire
+SWEEP_MODES = (0, 1, 3, 256)
 SWEEP_B = (1, 2, 3, 4, 5, 8, 9, 16, 24, 32, 33, 40, 48, 64, 96, 128, 130, 192, 256)
 SWEEP_H = tuple(range(16, 1025, 16))
 
@@ -37,8 +36,7 @@ def label(v, bwd):
         if not bwd:
             s += "/vec" if v["vec"] else "/scalar"
     elif v["gen"] == 2:
-        s = ("mma.sync", "mma.sync/every-warp-polls")[v["form"]] if bwd else ("mma.sync/v2", "mma.sync<1>",
-                                                                               "mma.sync<2>")[v["form"]]
+        s = "mma.sync" if bwd else ("mma.sync/v2", "mma.sync<1>", "mma.sync<2>")[v["form"]]
     else:
         s = "fma%dx%d" % (v["form"], v["R"]) + (("/vec" if v["vec"] else "/scalar") if bwd else "")
     return s + (" x%d" % v["nsplit"] if v["nsplit"] > 1 else "")

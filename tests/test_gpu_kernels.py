@@ -7,7 +7,7 @@ import torch.nn.functional as F
 
 from conftest import load_golden, rel_err, scaled_err
 from oracle import oracle_np as onp
-from oracle import lstm_ref, ref_port
+from oracle import ref_port
 from oracle.make_golden import AUDIO_CFG
 
 pytestmark = pytest.mark.gpu
@@ -257,9 +257,16 @@ def _check_bilstm(pkg, B, T, I, H, bidir, wtol=1e-4):
     (40, 9, 16, 512, False),    # unidirectional tensor-core plan (UB = 8), second batch group mostly padding rows
     (130, 5, 16, 512, True),    # more CTAs than SMs: three consecutive launches over 44-row blocks
     (64, 4, 24, 640, True),     # cfg D at batch 64: two launches of 32 rows
+    (64, 300, 64, 512, True),   # T = 300: 75 periods of the wgmma backward's 4-step generation tag
+    (64, 11, 24, 256, True),    # wgmma UB = 8: forward UBP 8, backward UB 8
+    (64, 11, 24, 384, True),    # wgmma forward UBP 12, backward UB 16 with a last n-block 128 wide
+    (64, 9, 16, 192, True),     # wgmma forward with UB = 6 (scalar publish), mma.sync backward
+    (64, 5, 16, 768, True),     # FMA forward over four launches, wgmma backward over two
+    (1, 9, 16, 512, True),      # a single batch row
+    (96, 5, 16, 512, True),     # wgmma forward and backward over two launches
 ])
 def test_bilstm_fwd_bwd_vs_aten_cpu(pkg, B, T, I, H, bidir):
-    _check_bilstm(pkg, B, T, I, H, bidir)
+    _check_bilstm(pkg, B, T, I, H, bidir, wtol=2e-4 if T > 100 else 1e-4)
 
 
 @pytest.mark.parametrize("B,T,I,H,bidir", [(32, 11, 24, 640, True), (64, 10, 120, 512, True), (130, 5, 16, 512, True)])
@@ -274,48 +281,15 @@ def test_bilstm_fp32_fma_kernels_on_the_large_shapes(pkg, B, T, I, H, bidir):
         lib.b200asr_debug_set_lstm_mode(0)
 
 
-@pytest.mark.parametrize("B,T,I,H,bidir", [(32, 11, 24, 640, True), (64, 10, 120, 512, True), (40, 9, 16, 512, False)])
+@pytest.mark.parametrize("B,T,I,H,bidir", [(32, 11, 24, 640, True), (64, 10, 120, 512, True), (40, 9, 16, 512, False),
+                                           (64, 300, 64, 512, True), (130, 5, 16, 512, True), (64, 11, 24, 384, True)])
 def test_bilstm_mma_sync_generation_on_the_large_shapes(pkg, B, T, I, H, bidir):
-    """The warp-level mma.sync 3xTF32 forward kernels (round 1) remain the path for shapes the wgmma kernel does
-    not take (H % 64 != 0 ...); keep them covered at the BASELINE shapes by forcing them (mode 3)."""
+    """The warp-level mma.sync 3xTF32 kernels (round 1) remain the path for shapes the wgmma kernels do not take
+    (H % 64 != 0 ...); keep them covered at the BASELINE shapes by forcing them (mode 3)."""
     lib = pkg.load_library()
     lib.b200asr_debug_set_lstm_mode(3)
     try:
         assert lib.b200asr_bilstm_uses_tcgen05(B, H, 2 if bidir else 1) == 0
-        _check_bilstm(pkg, B, T, I, H, bidir)
-    finally:
-        lib.b200asr_debug_set_lstm_mode(0)
-
-
-@pytest.mark.parametrize("B,T,I,H,bidir", [(64, 10, 120, 512, True), (40, 9, 16, 512, False), (64, 300, 64, 512, True)])
-def test_bilstm_backward_generation_toggle(pkg, B, T, I, H, bidir):
-    """Mode flag 512 selects the OTHER backward generation than the default one (wgmma <-> mma.sync): both stay
-    parity-tested at the BASELINE shape whichever is the default."""
-    lib = pkg.load_library()
-    lib.b200asr_debug_set_lstm_mode(512)
-    try:
-        _check_bilstm(pkg, B, T, I, H, bidir, wtol=2e-4 if T > 100 else 1e-4)
-    finally:
-        lib.b200asr_debug_set_lstm_mode(0)
-
-
-@pytest.mark.parametrize("B,T,I,H,bidir", [(64, 10, 120, 512, True), (32, 11, 24, 640, True), (40, 9, 16, 512, False),
-                                           (8, 13, 40, 320, True), (64, 300, 64, 512, True), (64, 11, 24, 256, True),
-                                           (64, 11, 24, 384, True)])
-def test_bilstm_exchange_protocol_toggle(pkg, B, T, I, H, bidir):
-    """Mode flags 1024 (forward) / 2048 (backward) select the OTHER state-exchange protocol of the wgmma kernels than
-    the default one (data-is-the-flag polling <-> fence + counter + bulk copy).  The flag-protocol backward keeps an
-    inbox of 32 x H floats in shared memory, so it has a plan only at H = 256, 384 and 512; at H = 640 and at
-    H = 320 the mode runs the backward of the other generation (asserted through the variant query).
-    tests/test_gpu_lstm_variants.py checks every protocol per batch row against float64."""
-    lib = pkg.load_library()
-    ndir = 2 if bidir else 1
-    fwd = lstm_ref.variant(lib, B, H, ndir, False, 1024 + 2048)
-    bwd = lstm_ref.variant(lib, B, H, ndir, True, 1024 + 2048)
-    assert fwd["gen"] == 1 and fwd["poll"] == 1
-    assert (bwd["gen"] == 1 and bwd["poll"] == 0) == (H in (256, 384, 512)), bwd
-    lib.b200asr_debug_set_lstm_mode(1024 + 2048)
-    try:
         _check_bilstm(pkg, B, T, I, H, bidir, wtol=2e-4 if T > 100 else 1e-4)
     finally:
         lib.b200asr_debug_set_lstm_mode(0)

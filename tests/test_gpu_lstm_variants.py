@@ -1,7 +1,7 @@
 """Every step-kernel variant of the persistent (Bi)LSTM recurrence, through the C ABI, against a float64 recurrence.
 
 The dispatcher (bilstm_run in csrc/lstm.cu) picks a kernel generation - wgmma with fp16 hi/lo operands, 3xTF32
-mma.sync, packed fp32 FMA - and within it a template instance, exchange protocol, loop form and number of launches.
+mma.sync, packed fp32 FMA - and within it a template instance, loop form and number of launches.
 It makes that choice through b200asr_debug_lstm_variant, so every case below asserts the variant it reaches, and one
 test checks that the cases together reach every code path a broad (B, H, ndir, mode) sweep of the query reaches.
 
@@ -52,14 +52,14 @@ CASES = [
     (64, 768, 2, 0, 5, "fma2x8 x4", "wgmma16/poll x2"),
     (32, 1024, 1, 0, 5, "fma2x8 x2", "fma2x8/vec x2"),                    # the RNN-LM layer
     (64, 512, 2, 256, 9, "wgmma16/flag+strict/vec", "wgmma16/poll"),
-    (64, 512, 2, 1024, 9, "wgmma16/poll/vec", "wgmma16/poll"),
-    (64, 384, 2, 1024, 9, "wgmma12/poll/vec", "wgmma16/poll"),
-    (64, 192, 2, 1024, 9, "wgmma8/poll/scalar", "mma.sync"),
-    (64, 256, 2, 2048, 9, "wgmma8/flag/vec", "wgmma8/flag"),
-    (64, 384, 2, 2048 + 256, 9, "wgmma12/flag+strict/vec", "wgmma16/flag+strict"),
-    (64, 512, 2, 2048, 9, "wgmma16/flag/vec", "wgmma16/flag"),
-    (64, 512, 2, 512, 9, "wgmma16/flag/vec", "mma.sync"),
+    (64, 256, 2, 256, 9, "wgmma8/flag+strict/vec", "wgmma8/poll"),        # strict acquire in every UBP instance,
+    (64, 384, 2, 256, 9, "wgmma12/flag+strict/vec", "wgmma16/poll"),      # with the scalar publish and over
+    (32, 640, 2, 256, 9, "wgmma12/flag+strict/scalar", "wgmma16/poll"),   # several launches
+    (130, 512, 2, 256, 5, "wgmma16/flag+strict/vec x3", "wgmma16/poll x3"),
+    (64, 448, 2, 0, 9, "wgmma16/flag/scalar", "mma.sync"),                # UB = 14 in the UBP = 16 instance
+    (64, 704, 2, 0, 5, "wgmma12/flag/scalar x2", "fma2x8/scalar x2"),
     (64, 512, 2, 3, 9, "mma.sync/v2", "mma.sync"),
+    (64, 640, 2, 3, 5, "mma.sync/v2 x2", "mma.sync x2"),
     (64, 192, 2, 3, 9, "mma.sync<2>", "mma.sync"),
     (64, 96, 2, 0, 9, "mma.sync<1>", "mma.sync"),
     (64, 480, 2, 3, 9, "mma.sync<1>", "mma.sync"),
@@ -200,10 +200,10 @@ def test_recurrence_vs_fp64_per_row(pkg, B, H, ndir, mode, T, fwd, bwd):
     print("variant %s | %s: worst row error %.3g (%.3g of the bound)" % (fwd, bwd, err, ratio))
 
 
-# (B, H, ndir, mode) of the time-edge, long-sequence, NaN and W_hh-scale cases: one per generation and protocol
+# (B, H, ndir, mode) of the time-edge, long-sequence, NaN and W_hh-scale cases: one per generation, and strict acquire
 EDGE_SHAPES = [
     (32, 256, 2, 0, "wgmma8/flag/vec", "wgmma8/poll"),
-    (32, 256, 2, 1024 + 2048, "wgmma8/poll/vec", "wgmma8/flag"),
+    (32, 256, 2, 256, "wgmma8/flag+strict/vec", "wgmma8/poll"),
     (32, 256, 2, 3, "mma.sync/v2", "mma.sync"),
     (32, 256, 2, 1, "fma1x4", "fma1x4/vec"),
 ]
@@ -212,7 +212,7 @@ EDGE_SHAPES = [
 @pytest.mark.parametrize("T", [1, 2, 5, 9, 17])
 @pytest.mark.parametrize("B,H,ndir,mode,fwd,bwd", EDGE_SHAPES, ids=[str(s[3]) for s in EDGE_SHAPES])
 def test_time_edges(pkg, B, H, ndir, mode, fwd, bwd, T):
-    """T across the 8-image ring of the forward polling exchange and the 4-step tag period of the backward one."""
+    """T across the two-image exchange of the flag protocol and the 4-step tag period of the polling backward."""
     assert _labels(pkg.load_library(), B, H, ndir, mode) == (fwd, bwd)
     _parity(pkg, B, H, ndir, mode, T, seed=100 + T, twice=False)
 
@@ -231,18 +231,15 @@ def test_whh_scale(pkg, B, H, ndir, mode, fwd, bwd, wscale):
     _parity(pkg, B, H, ndir, mode, 17, seed=11, wscale=wscale, twice=False)
 
 
-@pytest.mark.parametrize("B,H,ndir,mode,fwd,bwd", EDGE_SHAPES[:1] + EDGE_SHAPES[2:],
-                         ids=[str(s[3]) for s in EDGE_SHAPES[:1] + EDGE_SHAPES[2:]])
+@pytest.mark.parametrize("B,H,ndir,mode,fwd,bwd", EDGE_SHAPES, ids=[str(s[3]) for s in EDGE_SHAPES])
 def test_nan_stays_in_its_row(pkg, B, H, ndir, mode, fwd, bwd):
     """A NaN pre-activation in row 3 at frame 4 and a NaN dout in row 6 at frame 2: NaN exactly where float64 has it,
-    every other row within the bound.  Only the default exchange protocols: the forward polling protocol takes fp16
-    0xFFFF as 'not yet written' (DESIGN.md section 4)."""
-    assert lstm_ref.variant(pkg.load_library(), B, H, ndir, False, mode)["poll"] == 0
+    every other row within the bound."""
+    assert _labels(pkg.load_library(), B, H, ndir, mode) == (fwd, bwd)
     _parity(pkg, B, H, ndir, mode, 9, seed=13, pre_nan=(3, 4), dout_nan=(6, 2), twice=False)
 
 
-@pytest.mark.parametrize("mode,bwd", [(0, "wgmma8/poll"), (2048, "wgmma8/flag"), (3, "mma.sync"),
-                                      (1, "fma1x4/vec")])
+@pytest.mark.parametrize("mode,bwd", [(0, "wgmma8/poll"), (3, "mma.sync"), (1, "fma1x4/vec")])
 def test_huge_dout_row(pkg, mode, bwd):
     """A dout row at 2^105 (dG near 2^103): each generation keeps it finite and within the bound, like ATen.  The
     wgmma backward scales a row by 2^(13 - e) before its fp16 split; e must not be clamped below the row's exponent."""

@@ -28,21 +28,19 @@ def test_gpu_cases_reach_the_variants_they_name(pkg):
 
 
 @pytest.mark.parametrize("B,H,ndir,mode,fwd,bwd", [
-    # the flag-protocol backward needs an inbox of H * 32 * 4 bytes in shared memory: 2048 reaches it only up to
-    # H = 512; at H = 640 / 768 the mode falls back to the backward of the planner's other generation
-    (64, 256, 2, 2048, "wgmma8/flag/vec", "wgmma8/flag"),
-    (64, 384, 2, 2048, "wgmma12/flag/vec", "wgmma16/flag"),
-    (64, 512, 2, 2048, "wgmma16/flag/vec", "wgmma16/flag"),
-    (32, 640, 2, 2048, "wgmma12/flag/scalar", "mma.sync"),
-    (64, 768, 2, 2048, "fma2x8 x4", "fma2x8/vec x4"),
-    (32, 640, 2, 1024 + 2048, "wgmma12/poll/scalar", "mma.sync"),
     (64, 512, 2, 0, "wgmma16/flag/vec", "wgmma16/poll"),
     (64, 512, 2, 256, "wgmma16/flag+strict/vec", "wgmma16/poll"),      # strict acquire: flag protocol only
-    (64, 512, 2, 256 + 2048, "wgmma16/flag+strict/vec", "wgmma16/flag+strict"),
-    (64, 512, 2, 512, "wgmma16/flag/vec", "mma.sync"),
     (64, 512, 2, 3, "mma.sync/v2", "mma.sync"),
-    (64, 512, 2, 64 + 3, "mma.sync<2>", "mma.sync/every-warp-polls"),  # flag bit 2: first-generation MMA loops
     (64, 512, 2, 1, "fma2x8", "fma2x8/vec"),
+    (64, 256, 2, 256, "wgmma8/flag+strict/vec", "wgmma8/poll"),
+    (32, 640, 2, 0, "wgmma12/flag/scalar", "wgmma16/poll"),           # cfg D: the backward keeps no inbox in smem
+    (32, 640, 2, 256, "wgmma12/flag+strict/scalar", "wgmma16/poll"),
+    (32, 640, 2, 3, "mma.sync/v2", "mma.sync"),
+    (32, 640, 2, 1, "fma2x8", "fma2x8/scalar"),
+    (64, 768, 2, 0, "fma2x8 x4", "wgmma16/poll x2"),                  # no wgmma forward plan above H = 640 at B 64
+    (64, 768, 2, 3, "fma2x8 x4", "fma2x8/vec x4"),                    # ... and no mma.sync plan: mode 3 runs FMA
+    (32, 768, 2, 0, "fma2x8 x2", "wgmma16/poll"),
+    (64, 448, 2, 0, "wgmma16/flag/scalar", "mma.sync"),               # H % 128 != 0: no wgmma backward
     (3, 16, 2, 0, "fma1x4", "fma1x4/scalar"),
     (32, 1024, 1, 0, "fma2x8 x2", "fma2x8/vec x2"),
 ])

@@ -13,7 +13,7 @@ x = torch.randn(B, T, I, device="cuda", requires_grad=True)
 gy = torch.randn(B, T, 2 * H, device="cuda")
 lib = L.load()
 res = {}
-MODES = ((3, "mma.sync"), (0, "wgmma"), (512, "wgmma+bwd-toggle"), (3072, "wgmma+exchange-toggle"))
+MODES = ((3, "mma.sync"), (0, "wgmma"))
 if os.environ.get("ONLY_MODES"):
     MODES = tuple(m for m in MODES if str(m[0]) in os.environ["ONLY_MODES"].split(","))
 if os.environ.get("EXTRA_MODE"):
