@@ -127,8 +127,9 @@ class ASR(nn.Module):
 
 
 class Decoder(nn.Module):
-    """Speller: stacked LSTM stepped one token at a time + vocabulary projection (src/asr.py:158-221).
-    `self.layers` (nn.LSTM) is the parameter container; each step runs two GEMMs + the fused cell kernel."""
+    """Speller: stacked LSTM or GRU stepped one token at a time + vocabulary projection (src/asr.py:158-221).
+    `self.layers` (nn.LSTM / nn.GRU) is the parameter container; each step runs one GEMM + the fused cell kernel.
+    The hidden state is (h, c) for an LSTM and h alone for a GRU, each [layer, B, dim], as in the reference."""
 
     def __init__(self, input_dim, vocab_size, module, dim, layer, dropout):
         super().__init__()
@@ -137,45 +138,54 @@ class Decoder(nn.Module):
         self.dim = dim
         self.dropout = dropout
         assert module in ["LSTM", "GRU"], NotImplementedError
-        if module != "LSTM":
-            raise NotImplementedError("only an LSTM decoder is on the accelerated path")
+        self.module = module
         self.hidden_state = None
         self._dw = None
-        self.enable_cell = True
-        self.layers = nn.LSTM(input_dim, dim, num_layers=layer, dropout=dropout, batch_first=True)
+        self.enable_cell = module == "LSTM"
+        self.layers = getattr(nn, module)(input_dim, dim, num_layers=layer, dropout=dropout, batch_first=True)
         self.char_trans = nn.Linear(dim, vocab_size)
         self.final_dropout = nn.Dropout(dropout)
 
     def init_state(self, bs):
         self._dw = None          # per-batch handles of the own-GEMM step path (ops.decoder_weights)
         device = next(self.parameters()).device
-        self.hidden_state = (torch.zeros((self.layer, bs, self.dim), device=device),
-                             torch.zeros((self.layer, bs, self.dim), device=device))
+        if self.enable_cell:
+            self.hidden_state = (torch.zeros((self.layer, bs, self.dim), device=device),
+                                 torch.zeros((self.layer, bs, self.dim), device=device))
+        else:
+            self.hidden_state = torch.zeros((self.layer, bs, self.dim), device=device)
         return None  # the reference returns CPU copies here (a host sync) that ASR.forward never uses
 
     def set_state(self, hidden_state):
         device = next(self.parameters()).device
-        self.hidden_state = (hidden_state[0].to(device), hidden_state[1].to(device))
+        if self.enable_cell:
+            self.hidden_state = (hidden_state[0].to(device), hidden_state[1].to(device))
+        else:
+            self.hidden_state = hidden_state.to(device)
 
     def get_state(self):
-        return (self.hidden_state[0].cpu(), self.hidden_state[1].cpu())
+        if self.enable_cell:
+            return (self.hidden_state[0].cpu(), self.hidden_state[1].cpu())
+        return self.hidden_state.cpu()
 
     def get_query(self):
-        return self.hidden_state[0].transpose(0, 1).reshape(-1, self.dim * self.layer)
+        h = self.hidden_state[0] if self.enable_cell else self.hidden_state
+        return h.transpose(0, 1).reshape(-1, self.dim * self.layer)
 
     def project(self, x):
         return ops.linear3x(self.final_dropout(x), self.char_trans)
 
     def forward(self, x, project=True):
-        h_all, c_all = self.hidden_state
+        h_all, c_all = self.hidden_state if self.enable_cell else (self.hidden_state, None)
         hs, cs = [], []
         inp = x
         own = x.is_cuda and all(ops.decoder_gemm_supported(getattr(self.layers, "weight_ih_l%d" % l).shape[1], self.dim)
                                 for l in range(self.layer))
         if own and getattr(self, "_dw", None) is None:
-            # first step of a batch: [W_ih | W_hh] per layer + ONE weight-gradient accumulator node each
+            # first step of a batch: packed [W_ih | W_hh] per layer + ONE weight-gradient accumulator node each
             self._dw = [ops.decoder_weights(*(getattr(self.layers, "%s_l%d" % (n, l))
-                                              for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")))
+                                              for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")),
+                                            cell=self.module)
                         for l in range(self.layer)]
         for l in range(self.layer):
             w_ih = getattr(self.layers, "weight_ih_l%d" % l)
@@ -184,15 +194,20 @@ class Decoder(nn.Module):
             b_hh = getattr(self.layers, "bias_hh_l%d" % l)
             if own:
                 pre = ops.decoder_step(self._dw[l], inp, h_all[l])
-            else:
+            elif self.enable_cell:
                 pre = F.linear(inp, w_ih, b_ih) + F.linear(h_all[l], w_hh, b_hh)
-            h, c = ops.lstm_cell(pre, c_all[l])
+            else:
+                pre = ops.gru_preact(F.linear(inp, w_ih, b_ih), F.linear(h_all[l], w_hh, b_hh))
+            if self.enable_cell:
+                h, c = ops.lstm_cell(pre, c_all[l])
+                cs.append(c)
+            else:
+                h = ops.gru_cell(pre, h_all[l])
             hs.append(h)
-            cs.append(c)
             inp = h
             if self.dropout > 0 and l + 1 < self.layer:
                 inp = F.dropout(inp, self.dropout, self.training)
-        self.hidden_state = (torch.stack(hs, 0), torch.stack(cs, 0))
+        self.hidden_state = (torch.stack(hs, 0), torch.stack(cs, 0)) if self.enable_cell else torch.stack(hs, 0)
         out = inp
         char = self.project(out) if project else None
         return char, out

@@ -53,6 +53,8 @@ SIGNATURES = {
     "b200asr_debug_locattn_bwd_minb": (c_int, [c_int, c_int, c_int, c_int]),
     "b200asr_lstm_cell_fwd": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, _P]),
     "b200asr_lstm_cell_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P]),
+    "b200asr_gru_cell_fwd": (c_int, [_P, _P, _P, _P, c_int, c_int, _P]),
+    "b200asr_gru_cell_bwd": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, _P]),
     "b200asr_locattn_cluster_size": (c_int, [c_int, c_int]),
     "b200asr_locattn_wpart_floats": (c_size_t, [c_int, c_int, c_int]),
     "b200asr_locattn_fwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_float, c_int, c_int, c_int, c_int, c_int,

@@ -716,31 +716,105 @@ def lstm_cell(pre, c_prev):
     return LSTMCellFn.apply(pre, c_prev)
 
 
+class GRUCellFn(Function):
+    """Pointwise part of one GRU step (decoder, module: 'GRU'): pre [B, 4H] (r+z sums, gi_n, gh_n), h_prev -> h.
+    The backward returns dpre and only the direct part dh . z of dh_prev; the GEMM part comes back through pre."""
+
+    @staticmethod
+    def forward(ctx, pre, h_prev):
+        ctx.set_materialize_grads(False)
+        lib = L.load()
+        pre = _f32c(pre)
+        h_prev = _f32c(h_prev)
+        B, H4 = pre.shape
+        H = H4 // 4
+        assert H4 == 4 * H and tuple(h_prev.shape) == (B, H)
+        gates = torch.empty_like(pre)
+        h = torch.empty_like(h_prev)
+        L.check(lib.b200asr_gru_cell_fwd(L.ptr(pre), L.ptr(h_prev), L.ptr(gates), L.ptr(h), B, H, L.stream()),
+                "gru_cell_fwd")
+        ctx.save_for_backward(gates, h_prev)
+        return h
+
+    @staticmethod
+    def backward(ctx, dh):
+        lib = L.load()
+        gates, h_prev = ctx.saved_tensors
+        B, H = h_prev.shape
+        dh = _f32c(dh) if dh is not None else None
+        dpre = torch.empty_like(gates)
+        dhp = torch.empty_like(h_prev)
+        L.check(lib.b200asr_gru_cell_bwd(L.ptr(gates), L.ptr(h_prev), L.ptr(dh), L.ptr(dpre), L.ptr(dhp), B, H,
+                                         L.stream()), "gru_cell_bwd")
+        return dpre, dhp
+
+
+def gru_cell(pre, h_prev):
+    return GRUCellFn.apply(pre, h_prev)
+
+
+def gru_preact(gi, gh):
+    """The cell kernel's pre-activation layout from the two library products gi = x.W_ih^T + b_ih, gh = h.W_hh^T + b_hh
+    (each [B, 3H], r|z|n): [gh_rz + gi_rz, gi_n, gh_n] (the sum in ATen's operand order)."""
+    H2 = 2 * (gi.shape[1] // 3)
+    return torch.cat([gh[:, :H2] + gi[:, :H2], gi[:, H2:], gh[:, H2:]], 1)
+
+
 # ----------------------------------------------------------------------------------------------------------
 # Decoder LSTM step (src/asr.py:214-221): the two per-step projections  x . W_ih^T + h . W_hh^T + b  are ONE skinny
 # tensor-core GEMM on [x | h] . [W_ih | W_hh]^T (split-K, csrc/gemm.cu), the backward's input gradient is one more, and
 # the weight gradients of all L steps are ONE  dPre^T . [x | h]  contraction over the L*B stacked rows at the end of the
 # loop (same accumulator-node idea as the attention memory above) instead of 2 L library SGEMMs + 2 L accumulations.
+#
+# The GRU speller runs through the same step: its weights are packed so that one product yields the cell kernel's
+# layout (gru_cell),  Wcat [4H, I+H] = [[W_ir W_hr]; [W_iz W_hz]; [W_in 0]; [0 W_hn]],  bias = [b_r, b_z, b_in, b_hn]
+# with b_r = b_ir + b_hr, b_z = b_iz + b_hz.  The zero blocks cost 4/3 of the ideal FLOPs and weight bytes but keep
+# one launch per step in each direction (DESIGN §2.3 has the measurement against two products gi / gh).
 class DecMem:
     def __init__(self):
         self.dpre, self.x = [], []
 
 
+def pack_decoder_weights(cell, w_ih, w_hh, b_ih, b_hh):
+    """-> (wcat [4H, I+H], bias [4H]) of the step GEMM for an 'LSTM' or 'GRU' layer (PyTorch's gate order)."""
+    if cell == "LSTM":
+        return torch.cat([w_ih, w_hh], 1).contiguous(), (b_ih + b_hh).contiguous()
+    assert cell == "GRU"
+    H2, I = 2 * w_hh.shape[1], w_ih.shape[1]
+    wcat = torch.zeros((2 * H2, I + H2 // 2), device=w_ih.device, dtype=w_ih.dtype)
+    wcat[:H2, :I] = w_ih[:H2]
+    wcat[:H2, I:] = w_hh[:H2]
+    wcat[H2:H2 * 3 // 2, :I] = w_ih[H2:]
+    wcat[H2 * 3 // 2:, I:] = w_hh[H2:]
+    return wcat, torch.cat([b_ih[:H2] + b_hh[:H2], b_ih[H2:], b_hh[H2:]])
+
+
+def unpack_decoder_grads(cell, dW, db, I):
+    """Gradients of the packed (wcat, bias) -> (dW_ih, dW_hh, db_ih, db_hh) of the layer's parameters."""
+    if cell == "LSTM":
+        return dW[:, :I], dW[:, I:], db, db
+    H2 = dW.shape[0] // 2
+    H3 = H2 * 3 // 2
+    return (torch.cat([dW[:H2, :I], dW[H2:H3, :I]]), torch.cat([dW[:H2, I:], dW[H3:, I:]]),
+            db[:H3], torch.cat([db[:H2], db[H3:]]))
+
+
 class DecWeightsFn(Function):
     @staticmethod
-    def forward(ctx, mem, w_ih, w_hh, b_ih, b_hh):
+    def forward(ctx, mem, cell, w_ih, w_hh, b_ih, b_hh):
         ctx.set_materialize_grads(False)
         ctx.mem = mem
+        ctx.cell = cell
         ctx.I = w_ih.shape[1]
         token = torch.zeros(1, device=w_ih.device, dtype=torch.float32)
-        wcat = torch.cat([w_ih, w_hh], 1).contiguous()
+        wcat, bias = pack_decoder_weights(cell, w_ih, w_hh, b_ih, b_hh)
         wlo = tf32_residual(wcat)
         ctx.mark_non_differentiable(wlo)
-        return wcat, (b_ih + b_hh).contiguous(), token, wlo
+        return wcat, bias, token, wlo
 
     @staticmethod
     def backward(ctx, gW, gb, _gtoken, _gwlo=None):
-        mem, I = ctx.mem, ctx.I
+        mem = ctx.mem
         dW = gW
         db = gb
         if mem.dpre:
@@ -752,8 +826,8 @@ class DecWeightsFn(Function):
             db = s if gb is None else s + gb
             mem.dpre, mem.x = [], []
         if dW is None:
-            return None, None, None, None, None
-        return None, dW[:, :I], dW[:, I:], db, db
+            return None, None, None, None, None, None
+        return (None, None) + tuple(unpack_decoder_grads(ctx.cell, dW, db, ctx.I))
 
 
 class DecStepFn(Function):
@@ -779,14 +853,15 @@ class DecStepFn(Function):
         return None, torch.zeros(1, device=dpre.device), dx[:, :ctx.I], dx[:, ctx.I:], None, None, None
 
 
-def decoder_weights(w_ih, w_hh, b_ih, b_hh):
-    """-> (mem, wcat [4H, I+H], bias [4H], token) for decoder_step(); once per batch and decoder layer."""
+def decoder_weights(w_ih, w_hh, b_ih, b_hh, cell="LSTM"):
+    """-> (mem, wcat [4H, I+H], bias [4H], token) for decoder_step(); once per batch and decoder layer.
+    cell: 'LSTM' (pre feeds lstm_cell) or 'GRU' (pre feeds gru_cell)."""
     mem = DecMem()
-    return (mem,) + tuple(DecWeightsFn.apply(mem, w_ih, w_hh, b_ih, b_hh))
+    return (mem,) + tuple(DecWeightsFn.apply(mem, cell, w_ih, w_hh, b_ih, b_hh))
 
 
 def decoder_step(dw, x, h):
-    """pre-activations [B, 4H] of one decoder LSTM step from decoder_weights()' handle."""
+    """pre-activations [B, 4H] of one decoder LSTM or GRU step from decoder_weights()' handle."""
     mem, wcat, bias, token, wlo = dw
     return DecStepFn.apply(mem, token, x, h, wcat, bias, wlo)
 

@@ -161,6 +161,16 @@ B200ASR_API int b200asr_lstm_cell_bwd(const float* gates, const float* c_prev, c
                           const float* dc_next /* may be NULL */, float* dpreact, float* dc_prev, int B, int H,
                           b200asr_stream stream);
 
+/* ---- K13g: one GRU cell step (decoder with module: 'GRU', src/asr.py:214-221) ----------------------------------
+ * preact [B, 4H] = (gi_r + gh_r, gi_z + gh_z, gi_n, gh_n), gi = x.W_ih^T + b_ih, gh = h.W_hh^T + b_hh.
+ * r = sigmoid, z = sigmoid, n = tanh(gi_n + r.gh_n), h = (h_prev - n).z + n; gates [B, 4H] = (r, z, n, gh_n) (stash).
+ * Backward: dpreact [B, 4H] = (d pre_r, d pre_z, d gi_n, d gh_n), dh_prev = dh.z (the part that bypasses the GEMM).
+ * dh may be NULL (no gradient reaches h).                                                                           */
+B200ASR_API int b200asr_gru_cell_fwd(const float* preact, const float* h_prev, float* gates, float* h, int B, int H,
+                         b200asr_stream stream);
+B200ASR_API int b200asr_gru_cell_bwd(const float* gates, const float* h_prev, const float* dh /* may be NULL */,
+                         float* dpreact, float* dh_prev, int B, int H, b200asr_stream stream);
+
 /* ---- K12: location-aware attention step, forward and backward, one launch each ----------------------------------
  * replaces src/module.py:234-258 (LocationAwareAttention.forward) + :189-195 (_attend), single head:
  * Conv1d(1->K, 2R+1, pad R, no bias) over prev_att -> Linear(K->D, no bias) -> tanh -> energy = Linear(D->1)(tanh(key +
