@@ -2,7 +2,9 @@
 //
 // Restates /root/reference/src/solver.py:84-89 (clip_grad_norm_(params, 5.0); skip the step when the norm
 // is NaN) and the torch.optim.Adadelta / Adam updates selected by src/optim.py:33-52, but decides the
-// clip coefficient and the NaN skip on the device so the step needs no host synchronisation.
+// clip coefficient and the NaN skip on the device so the step needs no host synchronisation.  For the same
+// reason the count of applied steps (torch's state["step"], which a skipped step does not advance) lives on
+// the device, and Adam's bias corrections are formed there from it.
 #include "common.cuh"
 #include "../../include/b200asr.h"
 
@@ -44,18 +46,28 @@ __global__ void norm_final_kernel(const double* __restrict__ partials, int npart
     }
 }
 
+// The reference skips optimizer.step() exactly when math.isnan(norm).  An Inf norm is not skipped: clip_grad_norm_
+// scales by max_norm / (inf + 1e-6) = 0, so +-Inf gradient entries become NaN and every other entry 0.
 __device__ __forceinline__ bool clip_coef(const float* norm_dev, float max_norm, float* coef) {
     *coef = 1.f;
     if (!norm_dev) return true;
     const float nrm = *norm_dev;
-    if (!isfinite(nrm)) return false;  // reference skips optimizer.step() on a NaN norm
+    if (isnan(nrm)) return false;
     if (max_norm > 0.f) *coef = fminf(1.f, max_norm / (nrm + 1e-6f));
     return true;
 }
 
+// One thread, launched before the update kernel: the update reads the advanced count, as torch advances
+// state["step"] before it forms the bias corrections.
+__global__ void advance_step_kernel(const float* __restrict__ norm_dev, long long* __restrict__ step_count) {
+    if (!norm_dev || !isnan(*norm_dev)) *step_count += 1;
+}
+
+// rho / beta and their complements arrive rounded to fp32 once each, the complements formed in double on the host
+// (torch's `1 - rho` is a double scalar); 1.f - rho in fp32 would be off by up to 216 u for rho = 0.999.
 __global__ void __launch_bounds__(256) adadelta_kernel(float* __restrict__ p, const float* __restrict__ g,
                                                       float* __restrict__ sq, float* __restrict__ acc, long long n,
-                                                      float lr, float rho, float eps, float wd,
+                                                      float lr, float rho, float one_m_rho, float eps, float wd,
                                                       const float* __restrict__ norm_dev, float max_norm) {
     float coef;
     if (!clip_coef(norm_dev, max_norm, &coef)) return;
@@ -63,29 +75,33 @@ __global__ void __launch_bounds__(256) adadelta_kernel(float* __restrict__ p, co
         float gi = g[i] * coef;
         const float pi = p[i];
         if (wd != 0.f) gi = fmaf(wd, pi, gi);
-        const float s = rho * sq[i] + (1.f - rho) * gi * gi;
+        const float s = rho * sq[i] + one_m_rho * gi * gi;
         sq[i] = s;
         const float a = acc[i];
         const float delta = sqrtf(a + eps) / sqrtf(s + eps) * gi;
-        acc[i] = rho * a + (1.f - rho) * delta * delta;
+        acc[i] = rho * a + one_m_rho * delta * delta;
         p[i] = pi - lr * delta;
     }
 }
 
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g,
                                                   float* __restrict__ m, float* __restrict__ v, long long n, float lr,
-                                                  float beta1, float beta2, float eps, float wd, float bias1,
-                                                  float bias2, const float* __restrict__ norm_dev, float max_norm) {
+                                                  float beta1, float one_m_beta1, double beta1_d, float beta2,
+                                                  float one_m_beta2, double beta2_d, float eps, float wd,
+                                                  const long long* __restrict__ step_count,
+                                                  const float* __restrict__ norm_dev, float max_norm) {
     float coef;
     if (!clip_coef(norm_dev, max_norm, &coef)) return;
-    const float step_size = lr / bias1;
-    const float rsb2 = 1.f / sqrtf(bias2);
+    // bias corrections of the applied-step count in double, as torch forms them from its Python-float betas
+    const double t = (double)*step_count;
+    const float step_size = (float)((double)lr / (1.0 - pow(beta1_d, t)));
+    const float rsb2 = (float)(1.0 / sqrt(1.0 - pow(beta2_d, t)));
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         float gi = g[i] * coef;
         const float pi = p[i];
         if (wd != 0.f) gi = fmaf(wd, pi, gi);
-        const float mi = beta1 * m[i] + (1.f - beta1) * gi;
-        const float vi = beta2 * v[i] + (1.f - beta2) * gi * gi;
+        const float mi = beta1 * m[i] + one_m_beta1 * gi;
+        const float vi = beta2 * v[i] + one_m_beta2 * gi * gi;
         m[i] = mi;
         v[i] = vi;
         const float denom = sqrtf(vi) * rsb2 + eps;
@@ -121,27 +137,36 @@ static unsigned grid_for(long long n) {
     return (unsigned)b;
 }
 
+static int advance_step(const float* grad_norm, long long* step_count, cudaStream_t stream) {
+    advance_step_kernel<<<1, 1, 0, stream>>>(grad_norm, step_count);
+    B200_LAUNCH_CHECK("advance_step_kernel");
+    return B200_OK;
+}
+
 extern "C" int b200asr_adadelta_step(float* param, const float* grad, float* square_avg, float* acc_delta,
-                                     long long n, float lr, float rho, float eps, float weight_decay,
-                                     const float* grad_norm, float max_norm, b200asr_stream stream) {
-    B200_REQUIRE(param && grad && square_avg && acc_delta, "adadelta_step: null pointer");
-    if (n <= 0) return B200_OK;
-    adadelta_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(param, grad, square_avg, acc_delta, n, lr, rho, eps,
-                                                                  weight_decay, grad_norm, max_norm);
+                                     long long n, float lr, double rho, float eps, float weight_decay,
+                                     const float* grad_norm, float max_norm, long long* step_count,
+                                     b200asr_stream stream) {
+    B200_REQUIRE(param && grad && square_avg && acc_delta && step_count, "adadelta_step: null pointer");
+    const int rc = advance_step(grad_norm, step_count, (cudaStream_t)stream);
+    if (rc != B200_OK || n <= 0) return rc;
+    adadelta_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(param, grad, square_avg, acc_delta, n, lr,
+                                                                  (float)rho, (float)(1.0 - rho), eps, weight_decay,
+                                                                  grad_norm, max_norm);
     B200_LAUNCH_CHECK("adadelta_kernel");
     return B200_OK;
 }
 
 extern "C" int b200asr_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
-                                 float lr, float beta1, float beta2, float eps, float weight_decay, int step,
-                                 const float* grad_norm, float max_norm, b200asr_stream stream) {
-    B200_REQUIRE(param && grad && exp_avg && exp_avg_sq, "adam_step: null pointer");
-    B200_REQUIRE(step >= 1, "adam_step: step must be >= 1");
-    if (n <= 0) return B200_OK;
-    const float bias1 = 1.f - powf(beta1, (float)step);
-    const float bias2 = 1.f - powf(beta2, (float)step);
-    adam_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2,
-                                                              eps, weight_decay, bias1, bias2, grad_norm, max_norm);
+                                 float lr, double beta1, double beta2, float eps, float weight_decay,
+                                 const float* grad_norm, float max_norm, long long* step_count,
+                                 b200asr_stream stream) {
+    B200_REQUIRE(param && grad && exp_avg && exp_avg_sq && step_count, "adam_step: null pointer");
+    const int rc = advance_step(grad_norm, step_count, (cudaStream_t)stream);
+    if (rc != B200_OK || n <= 0) return rc;
+    adam_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(
+        param, grad, exp_avg, exp_avg_sq, n, lr, (float)beta1, (float)(1.0 - beta1), beta1, (float)beta2,
+        (float)(1.0 - beta2), beta2, eps, weight_decay, step_count, grad_norm, max_norm);
     B200_LAUNCH_CHECK("adam_kernel");
     return B200_OK;
 }

@@ -5,7 +5,7 @@ current CUDA stream. There is no CPU fallback - a missing library or a non-CUDA 
 """
 import ctypes
 import os
-from ctypes import c_int, c_float, c_longlong, c_size_t, c_void_p, c_char_p, c_ulonglong, POINTER
+from ctypes import c_int, c_float, c_double, c_longlong, c_size_t, c_void_p, c_char_p, c_ulonglong, POINTER
 
 import torch
 
@@ -82,9 +82,10 @@ SIGNATURES = {
     "b200asr_split_tf32": (c_int, [_P, _P, _P, c_longlong, _P]),
     "b200asr_grad_norm_scratch_bytes": (c_size_t, []),
     "b200asr_grad_norm": (c_int, [_P, c_longlong, _P, _P, _P]),
-    "b200asr_adadelta_step": (c_int, [_P, _P, _P, _P, c_longlong, c_float, c_float, c_float, c_float, _P, c_float, _P]),
-    "b200asr_adam_step": (c_int, [_P, _P, _P, _P, c_longlong, c_float, c_float, c_float, c_float, c_float, c_int, _P,
-                                  c_float, _P]),
+    "b200asr_adadelta_step": (c_int, [_P, _P, _P, _P, c_longlong, c_float, c_double, c_float, c_float, _P, c_float, _P,
+                                      _P]),
+    "b200asr_adam_step": (c_int, [_P, _P, _P, _P, c_longlong, c_float, c_double, c_double, c_float, c_float, _P,
+                                  c_float, _P, _P]),
 }
 
 

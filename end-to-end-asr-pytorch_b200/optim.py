@@ -3,7 +3,9 @@
 All parameters are re-pointed into one contiguous parameter buffer and all gradients into one contiguous gradient
 buffer, so that (i) the data-parallel exchange is ONE NCCL all-reduce of `flat_grad`, (ii) the global grad-norm is
 one reduction kernel and (iii) clip + NaN-skip + Adadelta/Adam is one fused update kernel that reads the norm on
-the device (no host sync in the step, unlike src/solver.py:84-89 which calls math.isnan on a Python float).
+the device (no host sync in the step, unlike src/solver.py:84-89 which calls math.isnan on a Python float).  The count
+of applied steps (torch's state["step"], which a skipped step does not advance) is a device counter for the same
+reason: only the device knows whether a step was skipped, also when the step is replayed from a CUDA graph.
 """
 from functools import partial
 
@@ -107,10 +109,15 @@ class Optimizer:
         dev = self.buf.flat.device
         self.state1 = torch.zeros_like(self.buf.flat)   # Adadelta square_avg / Adam exp_avg
         self.state2 = torch.zeros_like(self.buf.flat)   # Adadelta acc_delta  / Adam exp_avg_sq
-        self.n_steps = 0
+        self.step_count = torch.zeros(1, device=dev, dtype=torch.int64)   # applied updates, advanced on the device
         self.grad_norm = torch.zeros(1, device=dev, dtype=torch.float32)
         self._scratch = None
         self.pre_reduce = None    # hook: called with the flat gradient before the norm (data-parallel all-reduce)
+
+    @property
+    def n_steps(self):
+        """Number of applied updates (steps skipped on a NaN norm excluded); reading it synchronises the device."""
+        return int(self.step_count.item())
 
     # ---- reference API ----
     def get_opt_state_dict(self):
@@ -118,9 +125,10 @@ class Optimizer:
         s1, s2 = self.buf.views(self.state1), self.buf.views(self.state2)
         names = ("square_avg", "acc_delta") if self.opt_type == "Adadelta" else ("exp_avg", "exp_avg_sq")
         state = {}
-        if self.n_steps > 0:
+        n_steps = self.n_steps
+        if n_steps > 0:
             for i in range(len(self.buf.params)):
-                state[i] = {"step": torch.tensor(float(self.n_steps)), names[0]: s1[i].clone(), names[1]: s2[i].clone()}
+                state[i] = {"step": torch.tensor(float(n_steps)), names[0]: s1[i].clone(), names[1]: s2[i].clone()}
         group = {"lr": self.cur_lr, "eps": self.eps, "weight_decay": self.weight_decay,
                  "params": list(range(len(self.buf.params)))}
         if self.opt_type == "Adadelta":
@@ -136,7 +144,8 @@ class Optimizer:
             i = int(i)
             s1[i].copy_(st[names[0]])
             s2[i].copy_(st[names[1]])
-            self.n_steps = int(float(st.get("step", self.n_steps)))
+            if "step" in st:
+                self.step_count.fill_(int(float(st["step"])))
         if state_dict.get("param_groups"):
             self.cur_lr = state_dict["param_groups"][0].get("lr", self.cur_lr)
 
@@ -148,7 +157,8 @@ class Optimizer:
         return self.tf_rate(step)
 
     def step(self):
-        """grad-norm + clip(5.0) + NaN skip + update, all on the device; returns the norm (device scalar)."""
+        """grad-norm + clip(5.0) + NaN skip + update + step count, all on the device; returns the norm (device
+        scalar)."""
         lib = L.load()
         b = self.buf
         b.rebind_grads()
@@ -158,16 +168,16 @@ class Optimizer:
             self._scratch = torch.empty(lib.b200asr_grad_norm_scratch_bytes(), dtype=torch.uint8, device=b.flat.device)
         L.check(lib.b200asr_grad_norm(L.ptr(b.grad), b.total, L.ptr(self.grad_norm), L.ptr(self._scratch), L.stream()),
                 "grad_norm")
-        self.n_steps += 1
         if self.opt_type == "Adadelta":
             L.check(lib.b200asr_adadelta_step(L.ptr(b.flat), L.ptr(b.grad), L.ptr(self.state1), L.ptr(self.state2),
                                               b.total, self.cur_lr, self.rho, self.eps, self.weight_decay,
-                                              L.ptr(self.grad_norm), self.grad_clip, L.stream()), "adadelta_step")
+                                              L.ptr(self.grad_norm), self.grad_clip, L.ptr(self.step_count),
+                                              L.stream()), "adadelta_step")
         else:
             L.check(lib.b200asr_adam_step(L.ptr(b.flat), L.ptr(b.grad), L.ptr(self.state1), L.ptr(self.state2),
                                           b.total, self.cur_lr, self.betas[0], self.betas[1], self.eps,
-                                          self.weight_decay, self.n_steps, L.ptr(self.grad_norm), self.grad_clip,
-                                          L.stream()), "adam_step")
+                                          self.weight_decay, L.ptr(self.grad_norm), self.grad_clip,
+                                          L.ptr(self.step_count), L.stream()), "adam_step")
         return self.grad_norm
 
     def create_msg(self):

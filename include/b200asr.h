@@ -226,15 +226,21 @@ B200ASR_API int b200asr_embedding_bwd(const long long* ids, const float* dY, int
                                       void* workspace, size_t workspace_bytes, b200asr_stream stream);
 
 /* ---- K16: gradient norm, clip and optimizer update on flat buffers (src/solver.py:84-89, src/optim.py) ----
- * grad_norm (device scalar) may be NULL (no clipping, no NaN skip); max_norm <= 0 disables clipping.          */
+ * The norm is accumulated in fp64 and rounded once to fp32.  grad_norm (device scalar) may be NULL (no clipping,
+ * no skip); max_norm <= 0 disables clipping.  A NaN norm skips the update: nothing is written.  An Inf norm does
+ * not: the clip coefficient is max_norm / inf = 0, as in clip_grad_norm_.
+ * step_count (device int64) is the number of applied updates, torch.optim's state["step"]: each call advances it
+ * on the device unless the update is skipped, and Adam's bias corrections are formed from the advanced count in
+ * double.  rho / beta1 / beta2 are torch's double hyper-parameters; the kernels use them and their complements
+ * 1 - rho, 1 - beta formed in double, each rounded once to fp32.                                               */
 B200ASR_API size_t b200asr_grad_norm_scratch_bytes(void);
 B200ASR_API int b200asr_grad_norm(const float* grad, long long n, float* norm_out, void* scratch, b200asr_stream stream);
 B200ASR_API int b200asr_adadelta_step(float* param, const float* grad, float* square_avg, float* acc_delta, long long n,
-                          float lr, float rho, float eps, float weight_decay, const float* grad_norm,
-                          float max_norm, b200asr_stream stream);
+                          float lr, double rho, float eps, float weight_decay, const float* grad_norm,
+                          float max_norm, long long* step_count, b200asr_stream stream);
 B200ASR_API int b200asr_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n, float lr,
-                      float beta1, float beta2, float eps, float weight_decay, int step, const float* grad_norm,
-                      float max_norm, b200asr_stream stream);
+                      double beta1, double beta2, float eps, float weight_decay, const float* grad_norm,
+                      float max_norm, long long* step_count, b200asr_stream stream);
 
 /* ---- K6 / K9 / K11: dense  x . W^T (+ bias)  on the tensor cores at fp32-class accuracy ------------------------------
  * replaces the CTC head (src/asr.py:29,96), the proj_k / char_trans / pj Linear layers (src/asr.py:177,220,242-243;

@@ -518,8 +518,9 @@ def test_linear3x_matches_fp64_linear(pkg):
 
 
 # ------------------------------------------------------------------------------------------- optimizer
-def test_grad_norm_and_adadelta_vs_torch(pkg):
-    from ctypes import c_void_p
+def test_grad_norm_adadelta_and_step_count_vs_torch(pkg):
+    """The fused clip + Adadelta update (csrc/optim.cu) against torch.optim.Adadelta after clip_grad_norm_, 3 steps,
+    then the NaN-skip rule of src/solver.py:86-89; the device step count is torch's state["step"] throughout."""
     L = pkg.lib
     lib = L.load()
     torch.manual_seed(2)
@@ -531,13 +532,14 @@ def test_grad_norm_and_adadelta_vs_torch(pkg):
     sq = torch.zeros(n, device=DEV)
     acc = torch.zeros(n, device=DEV)
     norm = torch.zeros(1, device=DEV)
+    count = torch.zeros(1, dtype=torch.int64, device=DEV)
     scratch = torch.empty(lib.b200asr_grad_norm_scratch_bytes(), dtype=torch.uint8, device=DEV)
     pr = torch.nn.Parameter(p0.clone())
     opt = torch.optim.Adadelta([pr], lr=1.0, eps=1e-8)
     for it in range(3):
         L.check(lib.b200asr_grad_norm(L.ptr(g), n, L.ptr(norm), L.ptr(scratch), L.stream()))
         L.check(lib.b200asr_adadelta_step(L.ptr(p), L.ptr(g), L.ptr(sq), L.ptr(acc), n, 1.0, 0.9, 1e-8, 0.0,
-                                          L.ptr(norm), 5.0, L.stream()))
+                                          L.ptr(norm), 5.0, L.ptr(count), L.stream()))
         pr.grad = g0.clone()
         tn = torch.nn.utils.clip_grad_norm_([pr], 5.0)
         opt.step()
@@ -548,13 +550,14 @@ def test_grad_norm_and_adadelta_vs_torch(pkg):
     g[5] = float("nan")
     L.check(lib.b200asr_grad_norm(L.ptr(g), n, L.ptr(norm), L.ptr(scratch), L.stream()))
     L.check(lib.b200asr_adadelta_step(L.ptr(p), L.ptr(g), L.ptr(sq), L.ptr(acc), n, 1.0, 0.9, 1e-8, 0.0,
-                                      L.ptr(norm), 5.0, L.stream()))
+                                      L.ptr(norm), 5.0, L.ptr(count), L.stream()))
     assert torch.isnan(norm).item() and torch.equal(p, before)
+    assert count.item() == 3 == int(opt.state_dict()["state"][0]["step"])
 
 
-def test_grad_norm_and_adam_vs_torch(pkg):
+def test_grad_norm_adam_and_step_count_vs_torch(pkg):
     """The fused clip + Adam update (csrc/optim.cu) against torch.optim.Adam after clip_grad_norm_, 3 steps with bias
-    correction, then the NaN-skip rule of src/solver.py:86-89."""
+    correction, then the NaN-skip rule of src/solver.py:86-89 (the device step count does not advance)."""
     L = pkg.lib
     lib = L.load()
     torch.manual_seed(3)
@@ -564,6 +567,7 @@ def test_grad_norm_and_adam_vs_torch(pkg):
     m = torch.zeros(n, device=DEV)
     v = torch.zeros(n, device=DEV)
     norm = torch.zeros(1, device=DEV)
+    count = torch.zeros(1, dtype=torch.int64, device=DEV)
     scratch = torch.empty(lib.b200asr_grad_norm_scratch_bytes(), dtype=torch.uint8, device=DEV)
     pr = torch.nn.Parameter(p0.clone())
     opt = torch.optim.Adam([pr], lr=1e-3, betas=(0.9, 0.999), eps=1e-8)
@@ -571,8 +575,8 @@ def test_grad_norm_and_adam_vs_torch(pkg):
         g0 = torch.randn(n) * (0.01 if it == 1 else 3.0)         # step 1 is below the clip threshold
         g = g0.clone().to(DEV)
         L.check(lib.b200asr_grad_norm(L.ptr(g), n, L.ptr(norm), L.ptr(scratch), L.stream()))
-        L.check(lib.b200asr_adam_step(L.ptr(p), L.ptr(g), L.ptr(m), L.ptr(v), n, 1e-3, 0.9, 0.999, 1e-8, 0.0, it + 1,
-                                      L.ptr(norm), 5.0, L.stream()))
+        L.check(lib.b200asr_adam_step(L.ptr(p), L.ptr(g), L.ptr(m), L.ptr(v), n, 1e-3, 0.9, 0.999, 1e-8, 0.0,
+                                      L.ptr(norm), 5.0, L.ptr(count), L.stream()))
         pr.grad = g0.clone()
         tn = torch.nn.utils.clip_grad_norm_([pr], 5.0)
         opt.step()
@@ -581,9 +585,10 @@ def test_grad_norm_and_adam_vs_torch(pkg):
     before = p.clone()
     g[7] = float("nan")
     L.check(lib.b200asr_grad_norm(L.ptr(g), n, L.ptr(norm), L.ptr(scratch), L.stream()))
-    L.check(lib.b200asr_adam_step(L.ptr(p), L.ptr(g), L.ptr(m), L.ptr(v), n, 1e-3, 0.9, 0.999, 1e-8, 0.0, 4,
-                                  L.ptr(norm), 5.0, L.stream()))
+    L.check(lib.b200asr_adam_step(L.ptr(p), L.ptr(g), L.ptr(m), L.ptr(v), n, 1e-3, 0.9, 0.999, 1e-8, 0.0,
+                                  L.ptr(norm), 5.0, L.ptr(count), L.stream()))
     assert torch.isnan(norm).item() and torch.equal(p, before)
+    assert count.item() == 3 == int(opt.state_dict()["state"][0]["step"])
 
 
 def test_ctc_prefix_score_vs_reference_scorer(pkg):
