@@ -49,6 +49,7 @@
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/b200asr.h"
+#include "../../include/b200asr_debug.h"
 
 namespace b200asr {
 namespace {
@@ -464,13 +465,17 @@ int max_split(int M, int N) {
     return s < 1 ? 1 : (int)s;
 }
 
-int pick_split(int M, int N, int KB) {
+// Which rule decided the split count (b200asr_debug_gemm_plan reports it).
+enum SplitRule { SPLIT_ONE = 0, SPLIT_SM_FILL = 1, SPLIT_EFFICIENCY = 2, SPLIT_WORKSPACE = 3 };
+
+int pick_split(int M, int N, int KB, int* rule) {
     const int tiles = ((M + G_BM - 1) / G_BM) * ((N + G_BN - 1) / G_BN);
     const int sms = sm_count();
     int s = sms / tiles;
     if (s > KB / 8) s = KB / 8;           // at least 8 K blocks per slice
     if (s > G_MAX_SPLIT) s = G_MAX_SPLIT;
     if (s < 1) s = 1;
+    *rule = s > 1 ? SPLIT_SM_FILL : SPLIT_ONE;
     auto eff = [&](int q) {
         const long long ctas = (long long)tiles * q;
         return (double)ctas / (double)(((ctas + sms - 1) / sms) * sms);
@@ -478,9 +483,30 @@ int pick_split(int M, int N, int KB) {
     if (2 * tiles <= sms && eff(s) < 0.93) {
         const int cap = max_split(M, N);
         for (int q = s + 1; q <= cap && KB / q >= 64; ++q)
-            if (eff(q) >= 0.97) return q;
+            if (eff(q) >= 0.97) { *rule = SPLIT_EFFICIENCY; return q; }
     }
     return s;
+}
+
+// The split-K plan of one launch, for both kernels: the count pick_split asks for (counted in K blocks of 32 k, so the
+// f16x3 kernel's 64-k blocks count twice), one slice when the workspace cannot hold the partial tiles, slices of whole
+// units of `unit` K blocks (f16x3: one scale chunk), and no empty slices.
+struct SplitPlan {
+    int rule, requested, nsplit, kb_per_split;
+};
+
+SplitPlan plan_split(int M, int N, int KB, int unit, int rule_kb, size_t ws_bytes) {
+    SplitPlan p;
+    p.requested = pick_split(M, N, rule_kb, &p.rule);
+    int nsplit = p.requested;
+    if (nsplit > 1 && ws_bytes < (size_t)nsplit * M * N * sizeof(float)) {
+        nsplit = 1;
+        p.rule = SPLIT_WORKSPACE;
+    }
+    const int units = KB / unit;
+    p.kb_per_split = (units + nsplit - 1) / nsplit * unit;
+    p.nsplit = (KB + p.kb_per_split - 1) / p.kb_per_split;
+    return p;
 }
 
 // K blocks per accumulation chunk: B200ASR_GEMM_CHUNK = 1 | 2 | 4 (read once).  The tensor core truncates on every
@@ -498,10 +524,9 @@ int gemm_chunk() {
 template <bool A_MN, bool B_MN, bool B_PRE = false>
 int launch(const CUtensorMap& ma, const CUtensorMap& mb, GemmArgs g, void* ws, size_t ws_bytes, cudaStream_t stream,
            const CUtensorMap* mblo = nullptr) {
-    int nsplit = pick_split(g.M, g.N, g.KB);
-    if (nsplit > 1 && (ws == nullptr || ws_bytes < (size_t)nsplit * g.M * g.N * sizeof(float))) nsplit = 1;
-    g.kb_per_split = (g.KB + nsplit - 1) / nsplit;
-    nsplit = (g.KB + g.kb_per_split - 1) / g.kb_per_split;       // no empty slices
+    const SplitPlan p = plan_split(g.M, g.N, g.KB, 1, g.KB, ws ? ws_bytes : 0);
+    const int nsplit = p.nsplit;
+    g.kb_per_split = p.kb_per_split;
     g.partial = reinterpret_cast<float*>(ws);
     g.ch = gemm_chunk();
     const size_t smem = (size_t)GemmSmem<B_MN>::STAGES * GemmSmem<B_MN>::STAGE + 256;
@@ -910,10 +935,19 @@ extern "C" int b200asr_gemm3x_nt(const float* A, long long lda, long long a_bstr
     B200_REQUIRE(aligned16(A) && aligned16(B), "gemm3x_nt: operands must be 16-byte aligned");
     B200_REQUIRE(!permute_rows || (M % 4) == 0, "gemm3x_nt: the row permutation needs M %% 4 == 0");
     B200_REQUIRE(a_shift >= -G_BK && a_shift <= G_BK && b_shift >= -G_BK && b_shift <= G_BK, "gemm3x_nt: bad shift");
+    // Row r of an operand read with shift s belongs to step t = r - s only.  The last K block of a batch entry runs t
+    // up to the next multiple of 32, so with s < 0 the rows from T + s on would meet the other operand at a step t >= T
+    // (where it is not zero-filled when its shift is negative too): the tensor maps end at row T + min(s, 0).
+    const int Ta = T + (a_shift < 0 ? a_shift : 0), Tb = T + (b_shift < 0 ? b_shift : 0);
+    if (Ta <= 0 || Tb <= 0) {                                   // no step has both rows in range: an empty sum
+        if (!accumulate) B200_CUDA(cudaMemset2DAsync(C, (size_t)ldc * sizeof(float), 0, (size_t)N * sizeof(float), M,
+                                                      (cudaStream_t)stream));
+        return B200_OK;
+    }
     CUtensorMap ma, mb;
-    int rc = make_map_mn(&ma, A, M, T, batches, lda, a_bstride, true);
+    int rc = make_map_mn(&ma, A, M, Ta, batches, lda, a_bstride, true);
     if (rc != B200_OK) return rc;
-    rc = make_map_mn(&mb, B, N, T, batches, ldb, b_bstride, false);
+    rc = make_map_mn(&mb, B, N, Tb, batches, ldb, b_bstride, false);
     if (rc != B200_OK) return rc;
     GemmArgs g = {};
     g.C = C; g.M = M; g.N = N; g.ldc = ldc; g.accumulate = accumulate; g.perm = permute_rows;
@@ -1003,11 +1037,9 @@ extern "C" int b200asr_gemm_f16x3(const void* a_hi, const void* a_lo, const floa
     g.M = M; g.N = N; g.ldc = ldc; g.accumulate = accumulate; g.perm = permute_rows;
     g.KB = Kp / F_BK;
     // same split rule (and so the same workspace bound, b200asr_gemm3x_workspace_bytes) as the 3xTF32 kernel, in k
-    int nsplit = pick_split(M, N, Kp / G_BK);
-    if (nsplit > 1 && (workspace == nullptr || workspace_bytes < (size_t)nsplit * M * N * sizeof(float))) nsplit = 1;
-    const int chunks = g.KB / F_CH;
-    g.kb_per_split = (chunks + nsplit - 1) / nsplit * F_CH;
-    nsplit = (g.KB + g.kb_per_split - 1) / g.kb_per_split;
+    const SplitPlan p = plan_split(M, N, g.KB, F_CH, Kp / G_BK, workspace ? workspace_bytes : 0);
+    const int nsplit = p.nsplit;
+    g.kb_per_split = p.kb_per_split;
     g.partial = reinterpret_cast<float*>(workspace);
     const size_t smem = (size_t)F_STAGES * F_STAGE + 256;
     cudaStream_t st = (cudaStream_t)stream;
@@ -1022,5 +1054,29 @@ extern "C" int b200asr_gemm_f16x3(const void* a_hi, const void* a_lo, const floa
         gemm3x_reduce_kernel<<<blocks, 256, 0, st>>>(g.partial, nsplit, bias, C, M, N, ldc, accumulate, permute_rows);
         B200_LAUNCH_CHECK("gemm3x_reduce_kernel");
     }
+    return B200_OK;
+}
+
+extern "C" int b200asr_debug_gemm_plan(int form, int M, int N, int K, int batches, size_t workspace_bytes, int* desc) {
+    B200_REQUIRE(desc != nullptr && form >= 0 && form <= 4 && M > 0 && N > 0 && K > 0 && batches > 0 &&
+                     (form == 3 || batches == 1),
+                 "debug_gemm_plan: bad arguments (form %d M %d N %d K %d batches %d)", form, M, N, K, batches);
+    SplitPlan p;
+    int KB, ch, bk;
+    if (form == 4) {                                            // f16x3: 64-k blocks, one scale chunk per accumulation
+        bk = F_BK;
+        ch = F_CH;
+        KB = b200asr_f16x3_padded_k(K) / F_BK;
+        p = plan_split(M, N, KB, F_CH, KB * F_BK / G_BK, workspace_bytes);
+    } else {                                                    // 3xTF32: 32-k blocks; nt walks (batch, time)
+        bk = G_BK;
+        ch = gemm_chunk();
+        KB = (K + G_BK - 1) / G_BK * (form == 3 ? batches : 1);
+        p = plan_split(M, N, KB, 1, KB, workspace_bytes);
+    }
+    const int first = KB < p.kb_per_split ? KB : p.kb_per_split, last = KB - (p.nsplit - 1) * p.kb_per_split;
+    const int d[10] = {p.rule, p.requested, p.nsplit, p.kb_per_split, last, ch, (first - 1) % ch + 1,
+                       (last - 1) % ch + 1, KB, bk};
+    for (int i = 0; i < 10; ++i) desc[i] = d[i];
     return B200_OK;
 }

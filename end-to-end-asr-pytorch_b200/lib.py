@@ -51,6 +51,7 @@ SIGNATURES = {
     "b200asr_debug_lstm_variant": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_int)]),
     "b200asr_debug_ctc_variant": (c_int, [c_int]),
     "b200asr_debug_locattn_bwd_minb": (c_int, [c_int, c_int, c_int, c_int]),
+    "b200asr_debug_gemm_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_size_t, POINTER(c_int)]),
     "b200asr_lstm_cell_fwd": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, _P]),
     "b200asr_lstm_cell_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P]),
     "b200asr_gru_cell_fwd": (c_int, [_P, _P, _P, _P, c_int, c_int, _P]),

@@ -27,6 +27,14 @@ B200ASR_API int b200asr_debug_ctc_variant(int L_max);
 /* test: the minimum-blocks-per-SM instance (1 or 2) of the location-attention backward kernel that
  * b200asr_locattn_bwd(_acc) launches for these sizes on the current device; 0 for bad sizes. */
 B200ASR_API int b200asr_debug_locattn_bwd_minb(int B, int T, int D, int E);
+/* test: the split-K plan b200asr_gemm3x_tn (form 0; 1 with B_lo), _nn (2), _nt (3) or b200asr_gemm_f16x3 (4) makes
+ * for these sizes on the current device (132 SMs without one) with a workspace of workspace_bytes.  K is the
+ * contraction length (T for nt, which walks `batches` entries of T; batches must be 1 for the other forms; the
+ * unpadded or padded K for f16x3).  Fills desc[10] = {rule (0 one slice, 1 SM fill, 2 efficiency search, 3 workspace
+ * fallback), split count the rule asked for, slices launched, K blocks per slice, K blocks of the last slice,
+ * accumulation chunk length in K blocks, length of the last chunk of the first slice, of the last slice, K blocks in
+ * total, k per K block (32 for 3xTF32, 64 for f16x3)}.  The launchers make their choice through the same function. */
+B200ASR_API int b200asr_debug_gemm_plan(int form, int M, int N, int K, int batches, size_t workspace_bytes, int* desc);
 
 #ifdef __cplusplus
 }

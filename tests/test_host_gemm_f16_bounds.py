@@ -83,3 +83,31 @@ def test_scale_exponent_edges():
     e = _exp(amax)
     assert list(e) == [0, 0, 13, 126, -114]
     assert np.all(amax[:3] * np.exp2(e[:3]) >= 2.0 ** 13) and np.all(amax[:3] * np.exp2(e[:3]) < 2.0 ** 14)
+
+
+def _element_bound(a, b):
+    """The product terms of tests/test_gpu_gemm_parity.py's f16x3 bound: 3 * 2^-22 |a| |b| per product and
+    2^-37 * 128 cmax_a cmax_b per chunk (the emulation sums exactly, so the accumulation terms are left out)."""
+    a, b = a.astype(np.float64), b.astype(np.float64)
+    K = a.shape[1]
+    Kp = -(-K // CK) * CK
+    ap, bp = np.zeros((a.shape[0], Kp)), np.zeros((b.shape[0], Kp))
+    ap[:, :K], bp[:, :K] = np.abs(a), np.abs(b)
+    ca, cb = ap.reshape(len(a), -1, CK).max(2), bp.reshape(len(b), -1, CK).max(2)
+    return 3 * 2.0 ** -22 * (ap @ bp.T) + 2.0 ** -37 * CK * (ca @ cb.T)
+
+
+@pytest.mark.parametrize("case", ["rows", "chunks", "zero", "subnormal"])
+def test_per_element_bound(case):
+    """Every element of the emulated f16x3 product within half its own bound; one scale per tensor far outside it."""
+    a, b = _operands(case, np.random.default_rng(len(case)))
+    ref = a.astype(np.float64) @ b.astype(np.float64).T
+    bnd = _element_bound(a, b)
+    live = bnd > 0
+
+    def ratio(c):
+        assert np.all(c[~live] == 0)                 # zero rows: exactly zero
+        return float((np.abs(c - ref)[live] / bnd[live]).max())
+    assert ratio(_gemm(a, b)) <= 0.5
+    if case != "zero":
+        assert ratio(_gemm(a, b, per_tensor=True)) >= 4
