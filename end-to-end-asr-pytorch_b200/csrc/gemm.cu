@@ -7,6 +7,9 @@
 //                                                    that B can be read SHIFTED by one time step (dW_hh = dG^T . h_prev
 //                                                    without materialising h_prev: the row before the first / after the
 //                                                    last step of an utterance is out of bounds = zero-filled by TMA)
+//   conv mode (conv3x3_gemm_kernel, the same body): a 3x3 convolution over a zero-haloed channels-last buffer as an implicit GEMM - tn with the A
+//                     box of each 32-wide K block (one tap) loaded at that tap's row shift, nt (weight gradient) with
+//                     each B box at its tap's shift; see GemmArgs and b200asr_conv3x3_fwd / _wgrad (VGGExtractor)
 //   reference call sites: the input projection inside nn.LSTM (src/module.py:112-113,131), the CTC head (src/asr.py:29,
 //   96), proj_k / char_trans / pj (src/asr.py:242-243,177,220; src/module.py:123,155) and their autograd backward.
 //
@@ -83,6 +86,13 @@ struct GemmArgs {
     int kbt;               // K blocks per batch entry (MN-major operands walk (batch, time)); KB = batches * kbt
     int a_shift, b_shift;  // time shift of the rows read from A / B (nt form)
     int ch;                // K blocks per accumulation chunk
+    // Conv mode (CONV kernels): 3x3 convolution over a zero-haloed channels-last buffer [batches][T + 2][F + 2][C] as
+    // an implicit GEMM.  K = taps * C in (tap, channel) order; the K block at k reads tap k / cv_c, whose rows sit
+    // (tap / 3) (F + 2) + tap % 3 rows after the output row (tn: A rows; nt: B rows).  Output row m is the padded
+    // position m of the grid (t = (m / (F + 2)) % (T + 2), f = m % (F + 2)); rows with t >= T or f >= F are junk.
+    int cv_c, cv_fp, cv_t, cv_f;
+    int cv_relu;           // tn epilogue: + bias, then ReLU
+    const float* cv_mask;  // tn epilogue: zero where mask <= 0 (ReLU backward on the saved activation), pitch ldc
 };
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
@@ -273,13 +283,45 @@ __device__ __forceinline__ void store_acc(const float (&acc)[64], const float* b
     }
 }
 
+// Epilogue of the conv-mode tn form (never split): per output row of the grid, + bias, ReLU or the ReLU-backward mask,
+// and exact zeros on junk rows.  C (and the mask) are addressed at the row's zero-haloed position, so junk rows land on
+// the halo of the next buffer and keep it zero.  N % 4 == 0 (checked by the host).
+__device__ __forceinline__ void conv_store(const float (&acc)[64], const GemmArgs& g, int row0, int row1, int n0,
+                                           int lane) {
+    const int per = (g.cv_t + 2) * g.cv_fp;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int row = h ? row1 : row0;
+        if (row >= g.M) continue;
+        const int r = row % per, t = r / g.cv_fp, f = r - t * g.cv_fp;
+        const bool junk = t >= g.cv_t || f >= g.cv_f;
+        float* crow = g.C + (size_t)row * g.ldc;
+        const float* mrow = g.cv_mask ? g.cv_mask + (size_t)row * g.ldc : nullptr;
+#pragma unroll
+        for (int gq = 0; gq < 16; ++gq) {
+            const int n = n0 + 8 * gq + 2 * (lane & 3);
+            if (n >= g.N) continue;
+            float o0 = acc[4 * gq + 2 * h], o1 = acc[4 * gq + 2 * h + 1];
+            if (g.bias) { o0 += g.bias[n]; o1 += g.bias[n + 1]; }
+            if (g.cv_relu) { o0 = o0 < 0.f ? 0.f : o0; o1 = o1 < 0.f ? 0.f : o1; }    // NaN stays NaN, as clamp_min
+            if (mrow) {                                                               // as ATen's threshold_backward
+                const float2 mk = *reinterpret_cast<const float2*>(mrow + n);
+                o0 = mk.x <= 0.f ? 0.f : o0;
+                o1 = mk.y <= 0.f ? 0.f : o1;
+            }
+            if (junk) o0 = o1 = 0.f;
+            *reinterpret_cast<float2*>(crow + n) = make_float2(o0, o1);
+        }
+    }
+}
+
 // B_PRE: the residual of a K-major B comes from a pre-computed residual matrix (same shape / layout: the weights, split
 // once per step by b200asr_tf32_residual) through its own tensor map.  An MN-major B goes through the transposing
 // pass, which makes its residual in the same sweep.
-template <bool A_MN, bool B_MN, bool B_PRE>
-__global__ void __launch_bounds__(G_THREADS, 1)
-gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-              const __grid_constant__ CUtensorMap map_blo, const GemmArgs g) {
+// The kernel body, shared by gemm3x_kernel (the dense forms) and conv3x3_gemm_kernel (CONV: the conv mode).
+template <bool A_MN, bool B_MN, bool B_PRE, bool CONV>
+__device__ __forceinline__ void gemm3x_body(const CUtensorMap& map_a, const CUtensorMap& map_b,
+                                            const CUtensorMap& map_blo, const GemmArgs& g) {
     using L = GemmSmem<B_MN>;
     static_assert(!(B_PRE && B_MN), "only a K-major B brings a pre-computed residual");
     constexpr bool B_PREP = B_MN || !B_PRE;                        // warps 1..3 make B images
@@ -322,13 +364,22 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
                     uint8_t* st = smem + s * L::STAGE;
                     mbar_expect_tx(&full[s], a_bytes + (B_PRE ? 2 * b_bytes : b_bytes));
                     const int bt = kb / g.kbt, t0 = (kb - bt * g.kbt) * G_BK;
-                    if (A_MN) {
+                    if (CONV && !A_MN) {
+                        const int k = kb * G_BK, tap = k / g.cv_c;
+                        tma_load_2d(st, &map_a, k - tap * g.cv_c, m0 + (tap / 3) * g.cv_fp + tap % 3, &full[s]);
+                    } else if (A_MN) {
                         for (int j = 0; j < a_boxes; ++j)
                             tma_load_3d(st + j * G_BOX, &map_a, m0 + 32 * j, t0 + g.a_shift, bt, &full[s]);
                     } else {
                         tma_load_2d(st, &map_a, kb * G_BK, m0, &full[s]);
                     }
-                    if (B_MN) {
+                    if (CONV && B_MN) {
+                        for (int j = 0; j < b_boxes; ++j) {
+                            const int n = n0 + 32 * j, tap = n / g.cv_c;
+                            tma_load_3d(st + G_TILE + j * G_BOX, &map_b, n - tap * g.cv_c,
+                                        t0 + (tap / 3) * g.cv_fp + tap % 3, bt, &full[s]);
+                        }
+                    } else if (B_MN) {
                         for (int j = 0; j < b_boxes; ++j)
                             tma_load_3d(st + G_TILE + j * G_BOX, &map_b, n0 + 32 * j, t0 + g.b_shift, bt, &full[s]);
                     } else {
@@ -366,9 +417,27 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
 #pragma unroll
             for (int e = 0; e < 64; ++e) acc[e] += d[e];            // IEEE-add the chunk
         }
-        store_acc(acc, g.bias, g.C, g.partial, M, N, g.ldc, g.accumulate, g.perm,
-                  m0 + (A_MN ? mn_row(r0) : r0), m0 + (A_MN ? mn_row(r0 + 8) : r0 + 8), n0, lane);
+        if (CONV && !A_MN)
+            conv_store(acc, g, m0 + r0, m0 + r0 + 8, n0, lane);
+        else
+            store_acc(acc, g.bias, g.C, g.partial, M, N, g.ldc, g.accumulate, g.perm,
+                      m0 + (A_MN ? mn_row(r0) : r0), m0 + (A_MN ? mn_row(r0 + 8) : r0 + 8), n0, lane);
     }
+}
+
+template <bool A_MN, bool B_MN, bool B_PRE>
+__global__ void __launch_bounds__(G_THREADS, 1)
+gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+              const __grid_constant__ CUtensorMap map_blo, const GemmArgs g) {
+    gemm3x_body<A_MN, B_MN, B_PRE, false>(map_a, map_b, map_blo, g);
+}
+
+// Conv mode: WGRAD = false is the tn form (forward / input gradient), true the nt form (weight gradient).
+template <bool WGRAD>
+__global__ void __launch_bounds__(G_THREADS, 1)
+conv3x3_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                    const __grid_constant__ CUtensorMap map_blo, const GemmArgs g) {
+    gemm3x_body<WGRAD, WGRAD, false, true>(map_a, map_b, map_blo, g);
 }
 
 // C[perm(m)][n] (+)= bias[n] + sum_s partial[s][m][n]   (fixed summation order)
@@ -521,7 +590,7 @@ int gemm_chunk() {
     return ch;
 }
 
-template <bool A_MN, bool B_MN, bool B_PRE = false>
+template <bool A_MN, bool B_MN, bool B_PRE = false, bool CONV = false>
 int launch(const CUtensorMap& ma, const CUtensorMap& mb, GemmArgs g, void* ws, size_t ws_bytes, cudaStream_t stream,
            const CUtensorMap* mblo = nullptr) {
     const SplitPlan p = plan_split(g.M, g.N, g.KB, 1, g.KB, ws ? ws_bytes : 0);
@@ -530,11 +599,12 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mb, GemmArgs g, void* ws, s
     g.partial = reinterpret_cast<float*>(ws);
     g.ch = gemm_chunk();
     const size_t smem = (size_t)GemmSmem<B_MN>::STAGES * GemmSmem<B_MN>::STAGE + 256;
-    auto fn = gemm3x_kernel<A_MN, B_MN, B_PRE>;
+    static_assert(!CONV || (A_MN == B_MN && !B_PRE), "conv mode: tn or nt, no pre-split B");
+    auto fn = CONV ? conv3x3_gemm_kernel<A_MN> : gemm3x_kernel<A_MN, B_MN, B_PRE>;
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((g.N + G_BN - 1) / G_BN, (g.M + G_BM - 1) / G_BM, nsplit);
     fn<<<grid, G_THREADS, smem, stream>>>(ma, mb, mblo ? *mblo : mb, g);
-    B200_LAUNCH_CHECK("gemm3x_kernel");
+    B200_LAUNCH_CHECK(CONV ? "conv3x3_gemm_kernel" : "gemm3x_kernel");
     if (nsplit > 1) {
         const long long total = (long long)g.M * g.N;
         int blocks = (int)((total + 255) / 256);
@@ -954,6 +1024,58 @@ extern "C" int b200asr_gemm3x_nt(const float* A, long long lda, long long a_bstr
     g.kbt = (T + G_BK - 1) / G_BK; g.KB = g.kbt * batches;
     g.a_shift = a_shift; g.b_shift = b_shift;
     return launch<true, true>(ma, mb, g, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+// The zero-haloed layout of a 3x3 convolution's operands: grid rows R = batches (T + 2) (F + 2); a buffer holds R + F + 3
+// rows, position (b, t, f) of the data at grid row (b (T + 2) + t + 1) (F + 2) + f + 1 = m + F + 3.
+static int conv_geometry(const char* what, int C, int taps, int batches, int T, int F, int O, int* R) {
+    B200_REQUIRE((taps == 9 && C >= 32 && (C % 32) == 0) || (taps == 1 && C == 32),
+                 "%s: needs 9 taps over a multiple of 32 channels, or one tap over a 32-wide im2col (taps %d C %d)", what,
+                 taps, C);
+    B200_REQUIRE(batches > 0 && T > 0 && F > 0 && O > 0 && (O % 4) == 0,
+                 "%s: bad sizes batches=%d T=%d F=%d O=%d (O %% 4 must be 0)", what, batches, T, F, O);
+    const long long rows = (long long)batches * (T + 2) * (F + 2);
+    B200_REQUIRE(rows + F + 3 < (1LL << 31) - 4 * G_BM, "%s: too many rows (%lld)", what, rows);
+    *R = (int)rows;
+    return B200_OK;
+}
+
+extern "C" int b200asr_conv3x3_fwd(const float* x, int C, int taps, const float* w, const float* bias, const float* mask,
+                                   int relu, float* y, int batches, int T, int F, int O, b200asr_stream stream) {
+    B200_REQUIRE(x && w && y, "conv3x3_fwd: null pointer");
+    int R = 0;
+    int rc = conv_geometry("conv3x3_fwd", C, taps, batches, T, F, O, &R);
+    if (rc != B200_OK) return rc;
+    B200_REQUIRE(aligned16(x) && aligned16(w) && aligned16(y) && (!mask || aligned16(mask)),
+                 "conv3x3_fwd: operands must be 16-byte aligned");
+    const int K = taps * C, pad = F + 3;
+    CUtensorMap ma, mb;
+    if ((rc = make_map_k(&ma, x, taps == 9 ? R + pad : R, C, C, G_BM)) != B200_OK) return rc;
+    if ((rc = make_map_k(&mb, w, O, K, K, G_BN)) != B200_OK) return rc;
+    GemmArgs g = {};
+    g.bias = bias; g.C = y + (size_t)pad * O; g.M = R; g.N = O; g.ldc = O;
+    g.KB = K / G_BK; g.kbt = g.KB;
+    g.cv_c = C; g.cv_fp = F + 2; g.cv_t = T; g.cv_f = F; g.cv_relu = relu != 0;
+    g.cv_mask = mask ? mask + (size_t)pad * O : nullptr;
+    return launch<false, false, false, true>(ma, mb, g, nullptr, 0, (cudaStream_t)stream);
+}
+
+extern "C" int b200asr_conv3x3_wgrad(const float* dy, const float* x, int C, int taps, float* dw, int batches, int T,
+                                     int F, int O, void* workspace, size_t workspace_bytes, b200asr_stream stream) {
+    B200_REQUIRE(dy && x && dw, "conv3x3_wgrad: null pointer");
+    int R = 0;
+    int rc = conv_geometry("conv3x3_wgrad", C, taps, batches, T, F, O, &R);
+    if (rc != B200_OK) return rc;
+    B200_REQUIRE(aligned16(dy) && aligned16(x), "conv3x3_wgrad: operands must be 16-byte aligned");
+    const int pad = F + 3;
+    CUtensorMap ma, mb;
+    if ((rc = make_map_mn(&ma, dy + (size_t)pad * O, O, R, 1, O, 0, true)) != B200_OK) return rc;
+    if ((rc = make_map_mn(&mb, x, C, taps == 9 ? R + pad : R, 1, C, 0, false)) != B200_OK) return rc;
+    GemmArgs g = {};
+    g.C = dw; g.M = O; g.N = taps * C; g.ldc = taps * C;
+    g.kbt = (R + G_BK - 1) / G_BK; g.KB = g.kbt;
+    g.cv_c = C; g.cv_fp = F + 2; g.cv_t = T; g.cv_f = F;
+    return launch<true, true, false, true>(ma, mb, g, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int b200asr_tf32_residual(const float* x, float* lo, long long n, b200asr_stream stream) {

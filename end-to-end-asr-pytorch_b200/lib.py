@@ -74,6 +74,12 @@ SIGNATURES = {
     "b200asr_gemm3x_nt": (c_int, [_P, c_longlong, c_longlong, c_int, _P, c_longlong, c_longlong, c_int, _P, c_int, c_int,
                                   c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_tf32_residual": (c_int, [_P, _P, c_longlong, _P]),
+    "b200asr_conv3x3_fwd": (c_int, [_P, c_int, c_int, _P, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, _P]),
+    "b200asr_conv3x3_wgrad": (c_int, [_P, _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
+    "b200asr_vgg_im2col": (c_int, [_P, c_longlong, c_int, c_int, c_int, c_int, _P, _P]),
+    "b200asr_vgg_pool_fwd": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P]),
+    "b200asr_vgg_pool_bwd": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, _P]),
+    "b200asr_vgg_feat_grad": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P]),
     "b200asr_f16x3_padded_k": (c_int, [c_int]),
     "b200asr_f16x3_split_rows": (c_int, [_P, c_longlong, c_int, c_int, _P, _P, _P, _P]),
     "b200asr_f16x3_split_cols": (c_int, [_P, c_longlong, c_longlong, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),

@@ -5,8 +5,10 @@
                             the cuBLAS 3xTF32 composition when the input width is not a multiple of 4)
   LocationAwareAttention -> fused single-launch attention step (ops.loc_attention_step)
   CNNExtractor           -> its Conv1d(k 4, s 2) on the 3xTF32 GEMM kernel (ops.conv1d_k4s2p1)
-  VGGExtractor / ScaleDotAttention -> library convolutions / GEMMs (cuDNN, cuBLAS); these are
-      plain dense contractions outside the four north-star kernels (SURVEY.md 8(f) rank 4).
+  VGGExtractor           -> its 3x3 convolutions as implicit GEMMs on the 3xTF32 kernel, ReLU and max-pool fused
+                            (ops.vgg_extractor; the library sequence only for CPU tensors)
+  ScaleDotAttention      -> library GEMMs (cuBLAS): a plain dense contraction outside the four north-star kernels
+                            (SURVEY.md 8(f) rank 4).
 """
 import torch
 import torch.nn as nn
@@ -51,13 +53,10 @@ class VGGExtractor(nn.Module):
         return feature, feat_len
 
     def forward(self, feature, feat_len):
+        if feature.is_cuda:                     # implicit-GEMM convolutions + fused ReLU / max-pool (ops.VGGFn)
+            return ops.vgg_extractor(feature, feat_len, self.extractor, self.in_channel)
         feature, feat_len = self.view_input(feature, feat_len)
-        # Library convolutions, but NOT cuDNN's transform-domain algorithms: on zero-padded frames (exactly 0 activations,
-        # zero-initialised biases) Winograd / FFT tiles leave ~1e-9 rounding noise where the exact result is 0, ReLU'(x)
-        # then passes gradient where the reference's direct convolution blocks it (measured: the 64->128 / 128->128 bias
-        # gradients off by 5-20 %, tools/debug_vgg2.py).  ATen's native direct convolution matches the CPU path.
-        with torch.backends.cudnn.flags(enabled=False):
-            feature = self.extractor(feature)
+        feature = self.extractor(feature)
         feature = feature.transpose(1, 2)
         feature = feature.contiguous().view(feature.shape[0], feature.shape[1], self.out_dim)
         return feature, feat_len

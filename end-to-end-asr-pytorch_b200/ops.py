@@ -292,6 +292,146 @@ def conv1d_k4s2p1(x, conv):
     return conv(x.transpose(1, 2)).transpose(1, 2)
 
 
+def _vgg_buffer(B, T, F, C, device, zero_head=False):
+    """Zero-haloed channels-last buffer of a (T, F) activation: R = B (T+2) (F+2) grid rows plus F + 3 trailing rows
+    (include/b200asr.h).  zero_head zeroes the F + 3 rows in front of the first position, which a conv3x3_fwd output
+    does not write."""
+    buf = torch.empty((B * (T + 2) * (F + 2) + F + 3, C), device=device, dtype=torch.float32)
+    if zero_head:
+        buf[:F + 3].zero_()
+    return buf
+
+
+def conv3x3(x, C, taps, w, B, T, F, bias=None, mask=None, relu=False):
+    """3x3 convolution (padding 1) of the zero-haloed buffer x of (T, F) -> a new buffer of w.shape[0] channels: one
+    implicit-GEMM launch (b200asr_conv3x3_fwd); taps = 1 reads x as the first layer's [R, 32] im2col."""
+    lib = L.load()
+    O = w.shape[0]
+    y = _vgg_buffer(B, T, F, O, w.device, zero_head=True)
+    with L.timed("conv3x3_fwd", 4 * (x.numel() + w.numel() + y.numel() * (2 if mask is not None else 1))):
+        L.check(lib.b200asr_conv3x3_fwd(L.ptr(x), C, taps, L.ptr(w), L.ptr(bias), L.ptr(mask), int(relu), L.ptr(y), B,
+                                        T, F, O, L.stream()), "conv3x3_fwd")
+    return y
+
+
+def conv3x3_wgrad(dy, x, C, taps, B, T, F):
+    """dW [O, taps * C] (tap-major K) of a 3x3 convolution from the padded dY and its input buffer (b200asr_conv3x3_wgrad,
+    split-K over the grid rows)."""
+    lib = L.load()
+    O = dy.shape[1]
+    dw = torch.empty((O, taps * C), device=dy.device, dtype=torch.float32)
+    ws_bytes = lib.b200asr_gemm3x_workspace_bytes(O, taps * C)
+    ws = torch.empty(max(ws_bytes, 16), device=dy.device, dtype=torch.uint8)
+    with L.timed("conv3x3_wgrad", 4 * (dy.numel() + x.numel() + dw.numel())):
+        L.check(lib.b200asr_conv3x3_wgrad(L.ptr(dy), L.ptr(x), C, taps, L.ptr(dw), B, T, F, O, L.ptr(ws), ws_bytes,
+                                          L.stream()), "conv3x3_wgrad")
+    return dw
+
+
+def _vgg_taps(w):
+    """[O, C, 3, 3] -> [O, 9 C] with K = tap * C + c."""
+    return w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1).contiguous()
+
+
+def _vgg_taps_t(w):
+    """Weights of the input gradient: [O, C, 3, 3] -> [C, 9 O], flipped taps (w'[c][tap' O + o] = w[o][c][2-dt'][2-df'])."""
+    return w.detach().flip(2, 3).permute(1, 2, 3, 0).reshape(w.shape[1], -1).contiguous()
+
+
+def _vgg_untaps(dw, C):
+    """[O, 9 C] tap-major -> [O, C, 3, 3]."""
+    return dw.view(dw.shape[0], 3, 3, C).permute(0, 3, 1, 2).contiguous()
+
+
+class VGGFn(Function):
+    """VGGExtractor.extractor (src/module.py:7-66) on [B, T_in, Cin * F] features: T = T_in cropped to a multiple of 4,
+    2 x (conv3x3 -> ReLU -> conv3x3 -> ReLU -> MaxPool 2x2), output [B, T / 4, 128 * (F / 2 / 2)] with index c F' + f.
+    Each convolution, its input gradient and its weight gradient is one launch of the conv-mode 3xTF32 GEMM over
+    zero-haloed channels-last buffers (csrc/gemm.cu); bias + ReLU, the ReLU backward mask and the halo zeros are in its
+    epilogue.  The first conv (Cin <= 3) reads a staged [R, 32] im2col; max-pool forward / backward and the feature
+    gradient are csrc/vgg.cu; the bias gradients are column sums of the padded dY (zeros off the data)."""
+
+    @staticmethod
+    def forward(ctx, feature, Cin, w1, b1, w2, b2, w3, b3, w4, b4):
+        lib = L.load()
+        feature = _f32c(feature)
+        B, T_in, D = feature.shape
+        F = D // Cin
+        T = T_in - T_in % 4
+        T2, F2 = T // 2, F // 2
+        dev = feature.device
+        x0 = torch.empty((B * (T + 2) * (F + 2), 32), device=dev, dtype=torch.float32)
+        with L.timed("vgg_im2col", 4 * (B * T * D + x0.numel())):
+            L.check(lib.b200asr_vgg_im2col(L.ptr(feature), T_in * D, B, T, Cin, F, L.ptr(x0), L.stream()), "vgg_im2col")
+        wm1 = torch.zeros((w1.shape[0], 32), device=dev, dtype=torch.float32)
+        wm1[:, :9 * Cin] = _vgg_taps(w1)
+        y1 = conv3x3(x0, 32, 1, wm1, B, T, F, bias=_f32c(b1.detach()), relu=True)
+        y2 = conv3x3(y1, y1.shape[1], 9, _vgg_taps(w2), B, T, F, bias=_f32c(b2.detach()), relu=True)
+        p1 = _vgg_buffer(B, T2, F2, y2.shape[1], dev)
+        i1 = torch.empty((B, T2, F2, y2.shape[1]), device=dev, dtype=torch.uint8)
+        with L.timed("vgg_pool_fwd", 4 * (y2.numel() + p1.numel()) + i1.numel()):
+            L.check(lib.b200asr_vgg_pool_fwd(L.ptr(y2), B, T, F, y2.shape[1], L.ptr(p1), L.ptr(i1), 0, L.stream()),
+                    "vgg_pool_fwd")
+        y3 = conv3x3(p1, p1.shape[1], 9, _vgg_taps(w3), B, T2, F2, bias=_f32c(b3.detach()), relu=True)
+        y4 = conv3x3(y3, y3.shape[1], 9, _vgg_taps(w4), B, T2, F2, bias=_f32c(b4.detach()), relu=True)
+        C4 = y4.shape[1]
+        out = torch.empty((B, T2 // 2, C4 * (F2 // 2)), device=dev, dtype=torch.float32)
+        i2 = torch.empty((B, T2 // 2, F2 // 2, C4), device=dev, dtype=torch.uint8)
+        with L.timed("vgg_pool_fwd", 4 * (y4.numel() + out.numel()) + i2.numel()):
+            L.check(lib.b200asr_vgg_pool_fwd(L.ptr(y4), B, T2, F2, C4, L.ptr(out), L.ptr(i2), 1, L.stream()),
+                    "vgg_pool_fwd")
+        ctx.save_for_backward(x0, y1, y2, p1, y3, y4, i1, i2, w1, w2, w3, w4)
+        ctx.dims = (B, T_in, T, F, Cin)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = L.load()
+        x0, y1, y2, p1, y3, y4, i1, i2, w1, w2, w3, w4 = ctx.saved_tensors
+        B, T_in, T, F, Cin = ctx.dims
+        T2, F2 = T // 2, F // 2
+        dout = _f32c(dout)
+        dev = dout.device
+
+        def pool_bwd(dsrc, idx, y, T_, F_, flat):
+            dy = torch.empty_like(y)
+            with L.timed("vgg_pool_bwd", 4 * (dsrc.numel() + 2 * y.numel()) + idx.numel()):
+                L.check(lib.b200asr_vgg_pool_bwd(L.ptr(dsrc), L.ptr(idx), L.ptr(y), B, T_, F_, y.shape[1], L.ptr(dy),
+                                                 flat, L.stream()), "vgg_pool_bwd")
+            return dy
+
+        dy4 = pool_bwd(dout, i2, y4, T2, F2, 1)
+        dw4 = _vgg_untaps(conv3x3_wgrad(dy4, y3, y3.shape[1], 9, B, T2, F2), y3.shape[1])
+        dy3 = conv3x3(dy4, dy4.shape[1], 9, _vgg_taps_t(w4), B, T2, F2, mask=y3)
+        dw3 = _vgg_untaps(conv3x3_wgrad(dy3, p1, p1.shape[1], 9, B, T2, F2), p1.shape[1])
+        dp1 = conv3x3(dy3, dy3.shape[1], 9, _vgg_taps_t(w3), B, T2, F2)
+        dy2 = pool_bwd(dp1, i1, y2, T, F, 0)
+        dw2 = _vgg_untaps(conv3x3_wgrad(dy2, y1, y1.shape[1], 9, B, T, F), y1.shape[1])
+        dy1 = conv3x3(dy2, dy2.shape[1], 9, _vgg_taps_t(w2), B, T, F, mask=y1)
+        dw1 = conv3x3_wgrad(dy1, x0, 32, 1, B, T, F)[:, :9 * Cin]
+        dw1 = dw1.reshape(dw1.shape[0], 3, 3, Cin).permute(0, 3, 1, 2).contiguous()
+        dfeat = None
+        if ctx.needs_input_grad[0]:
+            dfeat = torch.empty((B, T_in, Cin * F), device=dev, dtype=torch.float32)
+            with L.timed("vgg_feat_grad", 4 * (dy1.numel() + dfeat.numel())):
+                L.check(lib.b200asr_vgg_feat_grad(L.ptr(dy1), L.ptr(_f32c(w1.detach())), B, T, T_in, Cin, F,
+                                                  w1.shape[0], L.ptr(dfeat), L.stream()), "vgg_feat_grad")
+        return (dfeat, None, dw1, dy1.sum(0), dw2, dy2.sum(0), dw3, dy3.sum(0), dw4, dy4.sum(0))
+
+
+def vgg_extractor(feature, feat_len, extractor, in_channel):
+    """VGGExtractor's forward on CUDA features [B, T_in, in_channel * F] -> ([B, T_in // 4, 128 * (F // 4)],
+    feat_len // 4).  Fewer than 4 frames cannot be convolved (the library path fails inside ATen): refused here, before
+    any launch."""
+    if feature.shape[1] < 4:
+        raise ValueError("VGGExtractor needs at least 4 frames per batch (time is cropped to a multiple of 4 and pooled "
+                         "twice); got a batch of %d frames" % feature.shape[1])
+    c1, c2, c3, c4 = extractor[0], extractor[2], extractor[5], extractor[7]
+    out = VGGFn.apply(feature, in_channel, c1.weight, c1.bias, c2.weight, c2.bias, c3.weight, c3.bias, c4.weight,
+                      c4.bias)
+    return out, feat_len // 4
+
+
 class Split:
     """fp32 matrix as (hi, lo) with hi exactly representable in TF32."""
 

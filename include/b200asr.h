@@ -285,6 +285,41 @@ B200ASR_API int b200asr_gemm3x_nt(const float* A, long long lda, long long a_bst
 /* B_lo of the tn form: lo[i] = x[i] - trunc_tf32(x[i]) over n floats. */
 B200ASR_API int b200asr_tf32_residual(const float* x, float* lo, long long n, b200asr_stream stream);
 
+/* ---- VGGExtractor (src/module.py:7-66): 3x3 convolutions as implicit GEMMs on the 3xTF32 kernel ----------------------
+ * Activations live in zero-haloed channels-last buffers of their (T, F): grid rows R = batches (T + 2) (F + 2), a buffer
+ * holds R + F + 3 rows of C floats, and position (b, t, f) sits at row m + F + 3 with m = (b (T + 2) + t) (F + 2) + f.
+ * conv3x3_fwd:  y at position (b, t, f), channel o  =  epilogue( bias[o] + sum_{tap, c} x[m + (tap / 3) (F + 2) + tap % 3][c]
+ *   * w[o][tap C + c] ),  tap = 3 dt + df.  taps = 9: x is a zero-haloed buffer, C a multiple of 32; taps = 1: x is the
+ *   first layer's im2col [R][32] (C = 32, b200asr_vgg_im2col) read at row m.  Epilogue: ReLU when relu != 0 (NaN stays
+ *   NaN); when mask != NULL (a buffer like y) zero where mask <= 0 (the ReLU backward of the layer that made mask).  Every
+ *   row from F + 3 on is written: junk grid rows (t >= T or f >= F) as exact zeros, which land on y's halo; the first
+ *   F + 3 rows of y must be zero beforehand.  The input gradient is the same call on the padded dY with the weights
+ *   flipped and transposed (w'[c][tap' O + o] = w[o][(8 - tap') C + c]).  One launch, no split-K.
+ * conv3x3_wgrad:  dw[o][tap C + c] = sum_m dy[m + F + 3][o] x[m + (tap / 3) (F + 2) + tap % 3][c]  (x as in _fwd; dy a
+ *   buffer with zeros on its halo), split-K over the rows with the workspace of b200asr_gemm3x_workspace_bytes(O,
+ *   taps C) (may be NULL).
+ * vgg_im2col: features (b, t, c, f) at feat[b ld_b + t Cin F + c F + f], Cin <= 3 -> the [R][32] im2col of the first
+ *   conv (k = tap Cin + c, zero beyond 9 Cin and on junk rows).
+ * vgg_pool_fwd: MaxPool2d(2, 2) of the buffer y of (T, F), T even, with ATen's scan order and NaN rule; idx [batches][T/2]
+ *   [F/2][C] (bytes) receives the window index 2 dt + df; out is the zero-haloed buffer of (T/2, F/2), every row
+ *   written, or when flat != 0 the prenet output [batches][T/2][C (F/2)] with index c (F/2) + f.
+ * vgg_pool_bwd: the gradient of the buffer y of (T, F) from dout (laid out as pool_fwd's out) through idx, zero where
+ *   y <= 0; every row of dy written.
+ * vgg_feat_grad: dfeat [batches][T_in][Cin F] from the first conv's padded dY and its weights w1 [O][Cin][3][3]; frames
+ *   t >= T get 0. */
+B200ASR_API int b200asr_conv3x3_fwd(const float* x, int C, int taps, const float* w, const float* bias, const float* mask,
+                        int relu, float* y, int batches, int T, int F, int O, b200asr_stream stream);
+B200ASR_API int b200asr_conv3x3_wgrad(const float* dy, const float* x, int C, int taps, float* dw, int batches, int T, int F,
+                          int O, void* workspace, size_t workspace_bytes, b200asr_stream stream);
+B200ASR_API int b200asr_vgg_im2col(const float* feat, long long ld_b, int batches, int T, int Cin, int F, float* out,
+                       b200asr_stream stream);
+B200ASR_API int b200asr_vgg_pool_fwd(const float* y, int batches, int T, int F, int C, float* out, unsigned char* idx,
+                         int flat, b200asr_stream stream);
+B200ASR_API int b200asr_vgg_pool_bwd(const float* dout, const unsigned char* idx, const float* y, int batches, int T, int F,
+                         int C, float* dy, int flat, b200asr_stream stream);
+B200ASR_API int b200asr_vgg_feat_grad(const float* dy1, const float* w1, int batches, int T, int T_in, int Cin, int F, int O,
+                          float* dfeat, b200asr_stream stream);
+
 /* ---- f16x3: the BiLSTM layer contractions on scaled fp16 hi/lo images (input width a multiple of 4) ----------------
  * An operand X[outer][k] (k = the contraction index) becomes two K-major fp16 images hi, lo [outer][Kp],
  * Kp = b200asr_f16x3_padded_k(K) (K rounded up to the 128-k scale chunk, zero-filled), and inverse scales
