@@ -254,7 +254,7 @@ class Attention(nn.Module):
         if self.key is None:
             self.att_layer.compute_mask(enc_feat, enc_len.to(enc_feat.device))
             self.key = torch.tanh(ops.linear3x(enc_feat, self.proj_k))
-            self.value = torch.tanh(self.proj_v(enc_feat)) if self.v_proj else enc_feat
+            self.value = torch.tanh(ops.linear3x(enc_feat, self.proj_v)) if self.v_proj else enc_feat
             if self.num_head > 1:
                 self.key = self.key.view(bs, ts, self.num_head, self.dim).permute(0, 2, 1, 3)
                 self.key = self.key.contiguous().view(bs * self.num_head, ts, self.dim)

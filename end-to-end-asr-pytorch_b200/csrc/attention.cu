@@ -51,9 +51,155 @@ struct AttnParams {
     float* wpart;         // [B*CS, P], P = D*K + K*W + D + 1   (d w_proj | d w_conv | d w_e | d b_e)
     int accumulate;       // != 0: d(key) and wpart are ADDED to (the decode loop's per-batch accumulators); dvalue may
                           // then be null (d(value) = sum over steps of attn (x) dctx is formed once after the loop)
+    int N;                // dot-product kernels: heads per utterance; row b is masked by len[b / N]
 };
 
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
+
+// ---- phases shared by the location-aware and the dot-product kernels -------------------------------------------
+// frame t's energy -> s_energy[t] of every CTA of the cluster
+__device__ __forceinline__ void energy_to_cluster(cg::cluster_group& cluster, float* s_energy, int rank, int CS, int t,
+                                                  float e) {
+    for (int rr = 0; rr < CS; ++rr) {
+        float* dst = (rr == rank) ? s_energy : cluster.map_shared_rank(s_energy, rr);
+        dst[t] = e;
+    }
+}
+
+// masked softmax over the full time axis (redundantly in every CTA; masked frames hold -inf and get exactly 0):
+// s_energy becomes the attention; attn_row (one CTA of the cluster) receives a copy
+__device__ __forceinline__ void softmax_in_place(float* s_energy, float* s_scratch, int T, float* attn_row) {
+    float mx = NEG_INF;
+    for (int t = threadIdx.x; t < T; t += blockDim.x) mx = fmaxf(mx, s_energy[t]);
+    mx = block_max(mx, s_scratch);
+    float sum = 0.f;
+    for (int t = threadIdx.x; t < T; t += blockDim.x) {
+        const float x = s_energy[t];
+        const float ex = (x == NEG_INF) ? 0.f : expf(x - mx);
+        s_energy[t] = ex;
+        sum += ex;
+    }
+    sum = block_sum(sum, s_scratch);
+    for (int t = threadIdx.x; t < T; t += blockDim.x) {
+        const float a = s_energy[t] / sum;
+        s_energy[t] = a;
+        if (attn_row) attn_row[t] = a;
+    }
+    __syncthreads();
+}
+
+// context slice of row b: ctx[e] for e in [rank*ES, (rank+1)*ES), frames t < len; float4 columns, time split across
+// thread groups, s_ctx [blockDim.x * 4] partial sums
+__device__ __forceinline__ void context_slice(const AttnParams& p, int b, int rank, int len, const float* s_attn,
+                                              float* s_ctx) {
+    const int T = p.T, E = p.E;
+    const int ES = E / p.CS;
+    const int ncol = ES >> 2;
+    const int cpp = min(ncol, (int)blockDim.x);          // columns per pass
+    const int ngroups = (int)blockDim.x / cpp;           // time groups
+    const int grp = threadIdx.x / cpp;
+    for (int cbase = 0; cbase < ncol; cbase += cpp) {
+        const int col = cbase + (threadIdx.x - grp * cpp);
+        const bool act = grp < ngroups && col < ncol;
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (act) {
+            const float* vb = p.value + (size_t)b * T * E + (size_t)rank * ES + col * 4;
+#pragma unroll 4
+            for (int t = grp; t < len; t += ngroups) {
+                const float a = s_attn[t];
+                const float4 v = *reinterpret_cast<const float4*>(vb + (size_t)t * E);
+                acc.x = fmaf(a, v.x, acc.x); acc.y = fmaf(a, v.y, acc.y);
+                acc.z = fmaf(a, v.z, acc.z); acc.w = fmaf(a, v.w, acc.w);
+            }
+        }
+        *reinterpret_cast<float4*>(s_ctx + (size_t)threadIdx.x * 4) = acc;
+        __syncthreads();
+        if (act && grp == 0) {
+            for (int g = 1; g < ngroups; ++g) {
+                const float4 o = *reinterpret_cast<const float4*>(s_ctx + (size_t)(g * cpp + col - cbase) * 4);
+                acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w;
+            }
+            *reinterpret_cast<float4*>(p.ctx + (size_t)b * E + (size_t)rank * ES + col * 4) = acc;
+        }
+        __syncthreads();
+    }
+}
+
+// backward, first phase: this CTA's feature slice of d(attn)[t] = dctx . value[b,t] for t < len, written into
+// s_part[rank*T + t] of every CTA of the cluster (plus d(value) = attn (x) dctx when p.dvalue is set).  One warp per
+// frame; the slice of d(ctx) is the same for every frame: registers; the value row of the NEXT frame of this warp is
+// loaded while the current one is reduced (one row per iteration left the loop bound by the load latency).
+// ES = E / CS <= 128 * MAXV.
+template <int MAXV>
+__device__ __forceinline__ void dattn_partials(const AttnParams& p, cg::cluster_group& cluster, int b, int rank, int len,
+                                               const float* s_attn, float* s_part) {
+    const int T = p.T, E = p.E, CS = p.CS;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    const int ES = E / CS;
+    const float* dcb = p.dctx + (size_t)b * E + (size_t)rank * ES;
+    const float* vb = p.value + (size_t)b * T * E + (size_t)rank * ES;
+    float4 dcr[MAXV], cur[MAXV], nxt[MAXV];
+#pragma unroll
+    for (int k = 0; k < MAXV; ++k) {
+        const int e = lane * 4 + 128 * k;
+        dcr[k] = (e < ES) ? *reinterpret_cast<const float4*>(dcb + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+        cur[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (warp < T && warp < len && e < ES)
+            cur[k] = *reinterpret_cast<const float4*>(vb + (size_t)warp * E + e);
+    }
+    for (int t = warp; t < T; t += nw) {
+        const float a = s_attn[t];
+        float* dvr = p.dvalue + ((size_t)b * T + t) * E + (size_t)rank * ES;
+        const int tn = t + nw;
+#pragma unroll
+        for (int k = 0; k < MAXV; ++k) {
+            const int e = lane * 4 + 128 * k;
+            nxt[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (tn < T && tn < len && e < ES)
+                nxt[k] = *reinterpret_cast<const float4*>(vb + (size_t)tn * E + e);
+        }
+        float part = 0.f;
+#pragma unroll
+        for (int k = 0; k < MAXV; ++k) {
+            const int e = lane * 4 + 128 * k;
+            if (e < ES) {
+                const float4 dc = dcr[k], v = cur[k];
+                if (t < len) part += dc.x * v.x + dc.y * v.y + dc.z * v.z + dc.w * v.w;
+                if (p.dvalue) {
+                    float4 dv = make_float4(0.f, 0.f, 0.f, 0.f);
+                    if (t < len) dv = make_float4(a * dc.x, a * dc.y, a * dc.z, a * dc.w);
+                    *reinterpret_cast<float4*>(dvr + e) = dv;
+                }
+            }
+            cur[k] = nxt[k];
+        }
+        part = warp_sum(part);
+        if (lane == 0) {
+            for (int rr = 0; rr < CS; ++rr) {
+                float* dst = (rr == rank) ? s_part : cluster.map_shared_rank(s_part, rr);
+                dst[rank * T + t] = part;
+            }
+        }
+    }
+}
+
+// backward, softmax phase (every CTA, full time axis, after the cluster barrier that completes dattn_partials):
+// g[t] = dattn[t] + sum of the CS partials; s_de[t] = attn[t] (g[t] - sum_t' attn g) / temperature for t < len, else 0
+__device__ __forceinline__ void softmax_bwd(const AttnParams& p, int b, int len, const float* s_attn, const float* s_part,
+                                            float* s_de, float* s_scratch) {
+    const int T = p.T, CS = p.CS;
+    float dot = 0.f;
+    for (int t = threadIdx.x; t < T; t += blockDim.x) {
+        float g = p.dattn ? p.dattn[(size_t)b * T + t] : 0.f;
+        for (int rr = 0; rr < CS; ++rr) g += s_part[rr * T + t];
+        s_de[t] = g;
+        if (t < len) dot = fmaf(s_attn[t], g, dot);
+    }
+    dot = block_sum(dot, s_scratch);
+    for (int t = threadIdx.x; t < T; t += blockDim.x)
+        s_de[t] = (t < len) ? s_attn[t] * (s_de[t] - dot) / p.temperature : 0.f;
+    __syncthreads();
+}
 
 // conv[k][tl] for the time range [t0, t0+nts) into s_conv[k*stride + tl]
 __device__ __forceinline__ void conv_slice(const float* s_prev, const float* s_w, float* s_conv, int K, int W,
@@ -75,7 +221,7 @@ __global__ void __launch_bounds__(1024) locattn_fwd_kernel(AttnParams p) {
     const int CS = p.CS;
     const int rank = (int)cluster.block_rank();
     const int b = blockIdx.x / CS;
-    const int T = p.T, D = p.D, E = p.E, K = p.K, R = p.R, W = 2 * R + 1;
+    const int T = p.T, D = p.D, K = p.K, R = p.R, W = 2 * R + 1;
     const int TS = (T + CS - 1) / CS;
     float* s_prev = sm;                    // [T + 2R]
     float* s_w = s_prev + T + 2 * R;       // [K*W]
@@ -130,65 +276,12 @@ __global__ void __launch_bounds__(1024) locattn_fwd_kernel(AttnParams p) {
             }
             e = (warp_sum(part) + be) / p.temperature;
         }
-        if (lane == 0) {
-            for (int rr = 0; rr < CS; ++rr) {
-                float* dst = (rr == rank) ? s_energy : cluster.map_shared_rank(s_energy, rr);
-                dst[t] = e;
-            }
-        }
+        if (lane == 0) energy_to_cluster(cluster, s_energy, rank, CS, t, e);
     }
     cluster.sync();
 
-    // masked softmax over the full time axis (redundantly in every CTA)
-    float mx = NEG_INF;
-    for (int t = threadIdx.x; t < T; t += blockDim.x) mx = fmaxf(mx, s_energy[t]);
-    mx = block_max(mx, s_scratch);
-    float sum = 0.f;
-    for (int t = threadIdx.x; t < T; t += blockDim.x) {
-        const float x = s_energy[t];
-        const float ex = (x == NEG_INF) ? 0.f : expf(x - mx);
-        s_energy[t] = ex;
-        sum += ex;
-    }
-    sum = block_sum(sum, s_scratch);
-    for (int t = threadIdx.x; t < T; t += blockDim.x) {
-        const float a = s_energy[t] / sum;
-        s_energy[t] = a;
-        if (rank == 0) p.attn[(size_t)b * T + t] = a;
-    }
-    __syncthreads();
-
-    // context slice: e in [rank*ES, (rank+1)*ES); float4 columns, time split across thread groups
-    const int ES = E / CS;
-    const int ncol = ES >> 2;
-    const int cpp = min(ncol, (int)blockDim.x);          // columns per pass
-    const int ngroups = (int)blockDim.x / cpp;           // time groups
-    const int grp = threadIdx.x / cpp;
-    for (int cbase = 0; cbase < ncol; cbase += cpp) {
-        const int col = cbase + (threadIdx.x - grp * cpp);
-        const bool act = grp < ngroups && col < ncol;
-        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (act) {
-            const float* vb = p.value + (size_t)b * T * E + (size_t)rank * ES + col * 4;
-#pragma unroll 4
-            for (int t = grp; t < len; t += ngroups) {
-                const float a = s_energy[t];
-                const float4 v = *reinterpret_cast<const float4*>(vb + (size_t)t * E);
-                acc.x = fmaf(a, v.x, acc.x); acc.y = fmaf(a, v.y, acc.y);
-                acc.z = fmaf(a, v.z, acc.z); acc.w = fmaf(a, v.w, acc.w);
-            }
-        }
-        *reinterpret_cast<float4*>(s_ctx + (size_t)threadIdx.x * 4) = acc;
-        __syncthreads();
-        if (act && grp == 0) {
-            for (int g = 1; g < ngroups; ++g) {
-                const float4 o = *reinterpret_cast<const float4*>(s_ctx + (size_t)(g * cpp + col - cbase) * 4);
-                acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w;
-            }
-            *reinterpret_cast<float4*>(p.ctx + (size_t)b * E + (size_t)rank * ES + col * 4) = acc;
-        }
-        __syncthreads();
-    }
+    softmax_in_place(s_energy, s_scratch, T, rank == 0 ? p.attn + (size_t)b * T : nullptr);
+    context_slice(p, b, rank, len, s_energy, s_ctx);
     cluster.sync();  // keep shared memory alive until every peer has finished its remote writes/reads
 }
 
@@ -204,7 +297,7 @@ __global__ void __launch_bounds__(MINB == 2 ? 384 : 512, MINB) locattn_bwd_kerne
     const int CS = p.CS;
     const int rank = (int)cluster.block_rank();
     const int b = blockIdx.x / CS;
-    const int T = p.T, D = p.D, E = p.E, K = p.K, R = p.R, W = 2 * R + 1;
+    const int T = p.T, D = p.D, K = p.K, R = p.R, W = 2 * R + 1;
     const int TS = (T + CS - 1) / CS;
     float* s_prev = sm;                          // [T + 2R]
     float* s_w = s_prev + T + 2 * R;             // [K*W]
@@ -235,69 +328,10 @@ __global__ void __launch_bounds__(MINB == 2 ? 384 : 512, MINB) locattn_bwd_kerne
     cluster.sync();  // all CTAs running + local init visible before any remote shared-memory access
 
     // A. d(attn) partial over my feature slice + d(value) = attn (x) dctx
-    const int ES = E / CS;
-    {
-        // the slice of d(ctx) is the same for every frame: registers; the value row of the NEXT frame of this warp is
-        // loaded while the current one is reduced (one row per iteration left the loop bound by the load latency)
-        constexpr int MAXV = MINB == 2 ? 4 : 8;              // ES <= 128 * MAXV (checked by the host wrapper)
-        const float* dcb = p.dctx + (size_t)b * E + (size_t)rank * ES;
-        float4 dcr[MAXV], cur[MAXV], nxt[MAXV];
-#pragma unroll
-        for (int k = 0; k < MAXV; ++k) {
-            const int e = lane * 4 + 128 * k;
-            dcr[k] = (e < ES) ? *reinterpret_cast<const float4*>(dcb + e) : make_float4(0.f, 0.f, 0.f, 0.f);
-            cur[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (warp < T && warp < len && e < ES)
-                cur[k] = *reinterpret_cast<const float4*>(p.value + ((size_t)b * T + warp) * E + (size_t)rank * ES + e);
-        }
-        for (int t = warp; t < T; t += nw) {
-            const float a = s_attn[t];
-            float* dvr = p.dvalue + ((size_t)b * T + t) * E + (size_t)rank * ES;
-            const int tn = t + nw;
-#pragma unroll
-            for (int k = 0; k < MAXV; ++k) {
-                const int e = lane * 4 + 128 * k;
-                nxt[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (tn < T && tn < len && e < ES)
-                    nxt[k] = *reinterpret_cast<const float4*>(p.value + ((size_t)b * T + tn) * E + (size_t)rank * ES + e);
-            }
-            float part = 0.f;
-#pragma unroll
-            for (int k = 0; k < MAXV; ++k) {
-                const int e = lane * 4 + 128 * k;
-                if (e < ES) {
-                    const float4 dc = dcr[k], v = cur[k];
-                    if (t < len) part += dc.x * v.x + dc.y * v.y + dc.z * v.z + dc.w * v.w;
-                    if (p.dvalue) {
-                        float4 dv = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (t < len) dv = make_float4(a * dc.x, a * dc.y, a * dc.z, a * dc.w);
-                        *reinterpret_cast<float4*>(dvr + e) = dv;
-                    }
-                }
-                cur[k] = nxt[k];
-            }
-            part = warp_sum(part);
-            if (lane == 0) {
-                for (int rr = 0; rr < CS; ++rr) {
-                    float* dst = (rr == rank) ? s_part : cluster.map_shared_rank(s_part, rr);
-                    dst[rank * T + t] = part;
-                }
-            }
-        }
-    }
+    dattn_partials<MINB == 2 ? 4 : 8>(p, cluster, b, rank, len, s_attn, s_part);   // ES <= 128 * MAXV (host-checked)
     cluster.sync();
     // B. softmax backward (every CTA, full time axis)
-    float dot = 0.f;
-    for (int t = threadIdx.x; t < T; t += blockDim.x) {
-        float g = p.dattn ? p.dattn[(size_t)b * T + t] : 0.f;
-        for (int rr = 0; rr < CS; ++rr) g += s_part[rr * T + t];
-        s_de[t] = g;
-        if (t < len) dot = fmaf(s_attn[t], g, dot);
-    }
-    dot = block_sum(dot, s_scratch);
-    for (int t = threadIdx.x; t < T; t += blockDim.x)
-        s_de[t] = (t < len) ? s_attn[t] * (s_de[t] - dot) / p.temperature : 0.f;
-    __syncthreads();
+    softmax_bwd(p, b, len, s_attn, s_part, s_de, s_scratch);
 
     // C. my time slice, in tiles of ATT_TT frames: recompute conv/loc/tanh, d(key), d(q), d(w_e), d(w_proj), d(conv)
     const int t0s = rank * TS;
@@ -441,14 +475,108 @@ __global__ void __launch_bounds__(256) attn_dvalue_kernel(const float* __restric
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// Scaled dot-product attention step (the reference's src/module.py:189-212, `_attend` + ScaleDotAttention.forward) on
+// rows b of B = utterances x heads, row b masked by len[b / N]:  e[t] = (q . key[b,t]) / temperature for t < len,
+// attn = softmax(e) over t < len (exactly 0 beyond), ctx = sum_t attn[t] value[b,t].  Same cluster split as the
+// location-aware kernels: the CS CTAs of a row split time for the energies and the feature axis for the context.
+__global__ void __launch_bounds__(512, 2) dotattn_fwd_kernel(AttnParams p) {
+    extern __shared__ __align__(16) float sm[];
+    __shared__ float s_scratch[32];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int CS = p.CS;
+    const int rank = (int)cluster.block_rank();
+    const int b = blockIdx.x / CS;
+    const int T = p.T, D = p.D;
+    const int TS = (T + CS - 1) / CS;
+    float* s_energy = sm;                        // [T]
+    float* s_ctx = sm + ((T + 3) & ~3);          // [blockDim.x * 4] partial sums, 16-B aligned
+
+    const int len = clampi((int)p.len[b / p.N], 0, T);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    float qv[16];                                // the row's query (D <= 512), lane-strided like the key rows
+#pragma unroll
+    for (int i = 0; i < 16; ++i) qv[i] = (lane + 32 * i < D) ? p.q[(size_t)b * D + lane + 32 * i] : 0.f;
+    cluster.sync();  // all CTAs of the cluster are running (required before any remote shared-memory access)
+
+    // energies of my time slice -> every CTA of the cluster
+    const int t0 = rank * TS;
+    for (int tl = warp; tl < TS; tl += nw) {
+        const int t = t0 + tl;
+        if (t >= T) break;
+        float e = NEG_INF;
+        if (t < len) {
+            const float* kr = p.key + ((size_t)b * T + t) * D;
+            float kv[16];                        // all loads of the frame's key row in flight at once
+#pragma unroll
+            for (int i = 0; i < 16; ++i) kv[i] = (lane + 32 * i < D) ? kr[lane + 32 * i] : 0.f;
+            float part = 0.f;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) part = fmaf(qv[i], kv[i], part);
+            e = warp_sum(part) / p.temperature;
+        }
+        if (lane == 0) energy_to_cluster(cluster, s_energy, rank, CS, t, e);
+    }
+    cluster.sync();  // the last remote access of this kernel: no peer touches this CTA's shared memory after it
+
+    softmax_in_place(s_energy, s_scratch, T, rank == 0 ? p.attn + (size_t)b * T : nullptr);
+    context_slice(p, b, rank, len, s_energy, s_ctx);
+}
+
+// Backward of one decode step on the per-batch accumulator (the decode loop's form, like b200asr_locattn_bwd_acc):
+// g[t] = dctx . value[b,t] + dattn[t], de[t] = attn[t] (g[t] - sum attn g) / temperature;  d(key)[b,t] += de[t] q for
+// t < len, dq_part[b, rank] = sum over my time slice of de[t] key[b,t].  No d(value): b200asr_attn_dvalue forms it
+// once after the loop.  MINB as in the location-aware backward: 2 (E / CS <= 512) when the CTAs outnumber the SMs.
+template <int MINB>
+__global__ void __launch_bounds__(MINB == 2 ? 384 : 512, MINB) dotattn_bwd_kernel(AttnParams p) {
+    extern __shared__ __align__(16) float sm[];
+    __shared__ float s_scratch[32];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int CS = p.CS;
+    const int rank = (int)cluster.block_rank();
+    const int b = blockIdx.x / CS;
+    const int T = p.T, D = p.D;
+    const int TS = (T + CS - 1) / CS;
+    float* s_q = sm;                             // [D]
+    float* s_attn = s_q + D;                     // [T]
+    float* s_de = s_attn + T;                    // [T]
+    float* s_part = s_de + T;                    // [CS*T] partial d(attn) of every peer
+
+    const int len = clampi((int)p.len[b / p.N], 0, T);
+    for (int i = threadIdx.x; i < D; i += blockDim.x) s_q[i] = p.q[(size_t)b * D + i];
+    for (int i = threadIdx.x; i < T; i += blockDim.x) s_attn[i] = p.attn_in[(size_t)b * T + i];
+    cluster.sync();  // all CTAs running + local init visible before any remote shared-memory access
+
+    dattn_partials<MINB == 2 ? 4 : 8>(p, cluster, b, rank, len, s_attn, s_part);
+    cluster.sync();  // the last remote access of this kernel
+    softmax_bwd(p, b, len, s_attn, s_part, s_de, s_scratch);
+
+    // my time slice: one thread per attention dim; frames t >= len are neither read nor written
+    const int t0s = rank * TS;
+    const int t1s = min(min(T, t0s + TS), len);
+    for (int d = threadIdx.x; d < D; d += blockDim.x) {
+        const float qd = s_q[d];
+        float acc = 0.f;
+#pragma unroll 4
+        for (int t = t0s; t < t1s; ++t) {
+            const float de = s_de[t];
+            const size_t off = ((size_t)b * T + t) * D + d;
+            acc = fmaf(de, p.key[off], acc);
+            p.dkey[off] += de * qd;
+        }
+        p.dq_part[((size_t)b * CS + rank) * D + d] = acc;
+    }
+}
+
 static int pick_cluster(int T, int E) {
     int cs = 4;
     while (cs > 1 && (E % (4 * cs) != 0 || T < 8 * cs)) cs >>= 1;
     return cs;
 }
 
-static int launch_attn(const void* fn, AttnParams& p, int threads, size_t smem, cudaStream_t stream) {
-    B200_REQUIRE(smem <= (size_t)max_optin_smem(), "loc_attention: %zu bytes of shared memory needed (T=%d D=%d too large)",
+static int launch_attn(const char* what, const void* fn, AttnParams& p, int threads, size_t smem,
+                       cudaStream_t stream) {
+    B200_REQUIRE(smem <= (size_t)max_optin_smem(), "%s: %zu bytes of shared memory needed (T=%d D=%d too large)", what,
                  smem, p.T, p.D);
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     cudaLaunchConfig_t cfg = {};
@@ -495,7 +623,7 @@ extern "C" int b200asr_locattn_fwd(const float* q, const float* key, const float
     const int W = 2 * R + 1, TS = (T + p.CS - 1) / p.CS;
     const size_t smem = sizeof(float) * ((size_t)T + 2 * R + (size_t)K * W + (size_t)D * K + 2 * D + T + (size_t)K * TS +
                                          (size_t)threads * 4 + 4);
-    return launch_attn((const void*)locattn_fwd_kernel, p, threads, smem, (cudaStream_t)stream);
+    return launch_attn("loc_attention", (const void*)locattn_fwd_kernel, p, threads, smem, (cudaStream_t)stream);
 }
 
 // MINB of the backward kernel: 2 when the CTAs outnumber the SMs and the smaller register budget fits the shape
@@ -534,8 +662,8 @@ static int locattn_bwd_impl(const float* q, const float* key, const float* value
                                          (size_t)p.CS * T + (size_t)K * ATT_TT + (size_t)ATT_TT * D +
                                          (size_t)K * (T + 2 * R));
     const bool two_per_sm = locattn_bwd_minb(B, T, D, E) == 2;
-    return launch_attn(two_per_sm ? (const void*)locattn_bwd_kernel<2> : (const void*)locattn_bwd_kernel<1>, p, threads,
-                       smem, (cudaStream_t)stream);
+    return launch_attn("loc_attention", two_per_sm ? (const void*)locattn_bwd_kernel<2> : (const void*)locattn_bwd_kernel<1>,
+                       p, threads, smem, (cudaStream_t)stream);
 }
 
 extern "C" int b200asr_locattn_bwd(const float* q, const float* key, const float* value, const float* prev_att,
@@ -566,4 +694,68 @@ extern "C" int b200asr_attn_dvalue(const float* attn_steps, const float* dctx_st
     attn_dvalue_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(attn_steps, dctx_steps, dvalue, B, L, T, E, accumulate);
     B200_LAUNCH_CHECK("attn_dvalue_kernel");
     return B200_OK;
+}
+
+// ---- scaled dot-product attention ----------------------------------------------------------------------------------
+// The limits of include/b200asr.h, checked before any CUDA call (ops.dot_attention_supported restates them).
+static int dotattn_check(const char* what, int R, int N, int T, int D, int E) {
+    B200_REQUIRE(R > 0 && N > 0 && T > 0 && D > 0 && E > 0 && R % N == 0,
+                 "%s: bad sizes R=%d N=%d T=%d D=%d E=%d (R must be a multiple of N)", what, R, N, T, D, E);
+    B200_REQUIRE(T <= B200ASR_DOTATTN_MAX_T, "%s: %d frames > %d", what, T, B200ASR_DOTATTN_MAX_T);
+    B200_REQUIRE(D <= 512, "%s: attention dim %d > 512", what, D);
+    B200_REQUIRE(E % 4 == 0, "%s: value dim %d must be a multiple of 4", what, E);
+    B200_REQUIRE(E / pick_cluster(T, E) <= 1024, "%s: value dim %d too large for %d-CTA clusters", what, E,
+                 pick_cluster(T, E));
+    return B200_OK;
+}
+
+static AttnParams dotattn_params(const float* q, const float* key, const float* value, const long long* enc_len,
+                                 int num_head, float temperature, int R, int T, int D, int E) {
+    AttnParams p = {};
+    p.q = q; p.key = key; p.value = value; p.len = enc_len; p.N = num_head; p.temperature = temperature;
+    p.B = R; p.T = T; p.D = D; p.E = E; p.CS = pick_cluster(T, E);
+    return p;
+}
+
+static int dotattn_bwd_minb(int R, int T, int E) {
+    const int cs = pick_cluster(T, E);
+    return ((long long)R * cs > sm_count() && E / cs <= 512) ? 2 : 1;
+}
+
+extern "C" int b200asr_dotattn_supported(int T, int D, int E) {
+    return T > 0 && T <= B200ASR_DOTATTN_MAX_T && D > 0 && D <= 512 && E > 0 && E % 4 == 0 &&
+           E / pick_cluster(T, E) <= 1024;
+}
+
+extern "C" int b200asr_debug_dotattn_bwd_minb(int R, int T, int E) {
+    return (R > 0 && T > 0 && E > 0) ? dotattn_bwd_minb(R, T, E) : 0;
+}
+
+extern "C" int b200asr_dotattn_fwd(const float* q, const float* key, const float* value, const long long* enc_len,
+                                   int num_head, float temperature, int R, int T, int D, int E, float* attn, float* ctx,
+                                   b200asr_stream stream) {
+    B200_REQUIRE(q && key && value && enc_len && attn && ctx, "dotattn_fwd: null pointer");
+    const int rc = dotattn_check("dotattn_fwd", R, num_head, T, D, E);
+    if (rc != B200_OK) return rc;
+    AttnParams p = dotattn_params(q, key, value, enc_len, num_head, temperature, R, T, D, E);
+    p.attn = attn; p.ctx = ctx;
+    const int threads = 512;
+    const size_t smem = sizeof(float) * (((size_t)T + 3) / 4 * 4 + (size_t)threads * 4);
+    return launch_attn("dotattn_fwd", (const void*)dotattn_fwd_kernel, p, threads, smem, (cudaStream_t)stream);
+}
+
+extern "C" int b200asr_dotattn_bwd_acc(const float* q, const float* key, const float* value, const long long* enc_len,
+                                       int num_head, float temperature, const float* attn, const float* dctx,
+                                       const float* dattn, int R, int T, int D, int E, float* dq_part, float* dkey_acc,
+                                       b200asr_stream stream) {
+    B200_REQUIRE(q && key && value && enc_len && attn && dctx && dq_part && dkey_acc, "dotattn_bwd_acc: null pointer");
+    const int rc = dotattn_check("dotattn_bwd_acc", R, num_head, T, D, E);
+    if (rc != B200_OK) return rc;
+    AttnParams p = dotattn_params(q, key, value, enc_len, num_head, temperature, R, T, D, E);
+    p.attn_in = attn; p.dctx = dctx; p.dattn = dattn; p.dq_part = dq_part; p.dkey = dkey_acc;
+    const bool two_per_sm = dotattn_bwd_minb(R, T, E) == 2;
+    const int threads = two_per_sm ? 384 : 512;
+    const size_t smem = sizeof(float) * ((size_t)D + 2 * (size_t)T + (size_t)p.CS * T);
+    return launch_attn("dotattn_bwd_acc", two_per_sm ? (const void*)dotattn_bwd_kernel<2> : (const void*)dotattn_bwd_kernel<1>,
+                       p, threads, smem, (cudaStream_t)stream);
 }

@@ -7,8 +7,8 @@
   CNNExtractor           -> its Conv1d(k 4, s 2) on the 3xTF32 GEMM kernel (ops.conv1d_k4s2p1)
   VGGExtractor           -> its 3x3 convolutions as implicit GEMMs on the 3xTF32 kernel, ReLU and max-pool fused
                             (ops.vgg_extractor; the library sequence only for CPU tensors)
-  ScaleDotAttention      -> library GEMMs (cuBLAS): a plain dense contraction outside the four north-star kernels
-                            (SURVEY.md 8(f) rank 4).
+  ScaleDotAttention      -> fused single-launch dot-product attention step, one or more heads
+                            (ops.dot_attention_mem_step; the library bmm sequence for CPU tensors and unsupported shapes)
 """
 import torch
 import torch.nn as nn
@@ -171,10 +171,24 @@ class BaseAttention(nn.Module):
 
 
 class ScaleDotAttention(BaseAttention):
-    """Scaled dot-product attention (src/module.py:198-212); library bmm path."""
+    """Scaled dot-product attention (src/module.py:198-212), one or more heads.  On CUDA tensors inside the kernels'
+    limits each step - energies, masked softmax, context - is ONE kernel launch on a per-batch attention memory
+    (ops.dot_attention_mem_step); the library bmm sequence remains for CPU tensors and unsupported shapes."""
+
+    def reset_mem(self):
+        super().reset_mem()
+        self._mem = None
 
     def forward(self, q, k, v):
         ts = k.shape[1]
+        if k.is_cuda and ops.dot_attention_supported(ts, k.shape[2], v.shape[2]):
+            if self._mem is None:
+                # first step of a batch: ONE gradient-accumulator node for key / value
+                self._mem = ops.attention_memory(k, v)
+            mem, mk, mv, token = self._mem
+            output, attn = ops.dot_attention_mem_step(mem, token, q, mk, mv, self.k_len, self.num_head,
+                                                      self.temperature)
+            return output, attn.view(-1, self.num_head, ts)
         energy = torch.bmm(q.unsqueeze(1), k.transpose(1, 2)).squeeze(1)
         output, attn = self._attend(energy, v)
         return output, attn.view(-1, self.num_head, ts)

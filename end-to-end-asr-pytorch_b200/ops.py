@@ -1114,10 +1114,11 @@ def loc_attention_step(q, key, value, prev_att, enc_len, conv_w, proj_w, e_w, e_
 # The decode loop calls the attention L times on the SAME key / value / weights (src/asr.py:112-151).  Left to autograd,
 # every step's backward writes a [B,T,D] and a [B,T,E] gradient that the engine then re-adds L-1 times (cfg C: 46 x
 # (78 + 11) MB written and ~3x that re-read and re-written by ATen adds).  Instead the per-batch gradients live in ONE
-# accumulator node:  AttnMemFn  hands key / value / the four small weights to the steps (plus a 1-element token whose
-# only job is to make the engine run AttnMemFn.backward after the LAST step);  LocAttnMemStepFn.backward  adds d(key) and
-# the weight-gradient partials in place (b200asr_locattn_bwd_acc) and records (attn_l, dctx_l);  AttnMemFn.backward
-# forms d(value) = sum_l attn_l (x) dctx_l once (b200asr_attn_dvalue) and reduces the weight partials once.
+# accumulator node:  AttnMemFn  hands key / value / the location weights (none for the dot-product attention) to the
+# steps (plus a 1-element token whose only job is to make the engine run AttnMemFn.backward after the LAST step);  the
+# step's backward (LocAttnMemStepFn / DotAttnMemStepFn) adds d(key) - and the location weights' partials - in place
+# (b200asr_locattn_bwd_acc / b200asr_dotattn_bwd_acc) and records (attn_l, dctx_l);  AttnMemFn.backward forms
+# d(value) = sum_l attn_l (x) dctx_l once (b200asr_attn_dvalue) and reduces the weight partials once.
 class AttnMem:
     def __init__(self):
         self.dkey = None
@@ -1128,19 +1129,19 @@ class AttnMem:
 
 class AttnMemFn(Function):
     @staticmethod
-    def forward(ctx, mem, key, value, conv_w, proj_w, e_w, e_b):
+    def forward(ctx, mem, key, value, *loc_w):
         ctx.set_materialize_grads(False)        # undefined output gradients arrive as None, not as [B,T,E] zeros
         ctx.mem = mem
-        ctx.shapes = (key.shape, value.shape, conv_w.shape, proj_w.shape, e_w.shape, e_b.shape)
+        ctx.shapes = (key.shape, value.shape) + tuple(w.shape for w in loc_w)
         token = torch.zeros(1, device=key.device, dtype=torch.float32)
-        return (key.view_as(key), value.view_as(value), conv_w.view_as(conv_w), proj_w.view_as(proj_w),
-                e_w.view_as(e_w), e_b.view_as(e_b), token)
+        return (key.view_as(key), value.view_as(value)) + tuple(w.view_as(w) for w in loc_w) + (token,)
 
     @staticmethod
-    def backward(ctx, gkey, gvalue, gcw, gpw, gew, geb, _gtoken):
+    def backward(ctx, gkey, gvalue, *grads):
         lib = L.load()
         mem = ctx.mem
-        s_key, s_value, s_conv, s_proj, s_ew, s_eb = ctx.shapes
+        s_key, s_value = ctx.shapes[:2]
+        g_loc, _gtoken = grads[:-1], grads[-1]
         B, T, D = s_key
         E = s_value[2]
         dev = _gtoken.device
@@ -1158,24 +1159,27 @@ class AttnMemFn(Function):
                                                 int(acc), L.stream()), "attn_dvalue")
         else:
             dvalue = gvalue
-        d_conv = d_proj = d_ew = d_eb = None
+        d_loc = (None,) * len(g_loc)
         if mem.wpart is not None:
+            s_conv, s_proj, s_ew, s_eb = ctx.shapes[2:]
             K, _, W = s_conv
             wsum = mem.wpart.sum(0)
-            d_proj = wsum[:D * K].view(s_proj)
-            d_conv = wsum[D * K:D * K + K * W].view(s_conv)
-            d_ew = wsum[D * K + K * W:D * K + K * W + D].view(s_ew)
-            d_eb = wsum[D * K + K * W + D:].view(s_eb)
+            d_loc = (wsum[D * K:D * K + K * W].view(s_conv), wsum[:D * K].view(s_proj),
+                     wsum[D * K + K * W:D * K + K * W + D].view(s_ew), wsum[D * K + K * W + D:].view(s_eb))
         add = lambda a, b: a if b is None else (b if a is None else a + b)
         mem.dkey = mem.wpart = None
         mem.attn, mem.dctx = [], []
-        return None, dkey, dvalue, add(d_conv, gcw), add(d_proj, gpw), add(d_ew, gew), add(d_eb, geb)
+        return (None, dkey, dvalue) + tuple(add(d, g) for d, g in zip(d_loc, g_loc))
 
 
-def attention_memory(key, value, conv_w, proj_w, e_w, e_b):
-    """-> (mem, key, value, conv_w, proj_w, e_w, e_b, token) for loc_attention_mem_step."""
+def attention_memory(key, value, conv_w=None, proj_w=None, e_w=None, e_b=None):
+    """-> (mem, key, value, conv_w, proj_w, e_w, e_b, token) for loc_attention_mem_step, or, without the location
+    weights, (mem, key, value, token) for dot_attention_mem_step."""
     mem = AttnMem()
-    return (mem,) + tuple(AttnMemFn.apply(mem, _f32c(key), _f32c(value), conv_w, proj_w, e_w, e_b))
+    loc_w = tuple(w for w in (conv_w, proj_w, e_w, e_b) if w is not None)
+    if len(loc_w) not in (0, 4):
+        raise ValueError("attention_memory: pass all four location weights or none")
+    return (mem,) + tuple(AttnMemFn.apply(mem, _f32c(key), _f32c(value), *loc_w))
 
 
 class LocAttnMemStepFn(Function):
@@ -1238,6 +1242,75 @@ class LocAttnMemStepFn(Function):
 def loc_attention_mem_step(mem, token, q, key, value, prev_att, enc_len, conv_w, proj_w, e_w, e_b, temperature):
     """-> (context [B,E], attn [B,T]); key ... e_b and token come from attention_memory()."""
     return LocAttnMemStepFn.apply(mem, token, q, key, value, prev_att, enc_len, conv_w, proj_w, e_w, e_b, temperature)
+
+
+# ----------------------------------------------------------------------------------------------------------
+DOTATTN_MAX_T = 8192          # B200ASR_DOTATTN_MAX_T of include/b200asr.h
+
+
+def dot_attention_supported(T, D, E):
+    """The limits of b200asr_dotattn_fwd / _bwd_acc (include/b200asr.h; cluster rule of b200asr_locattn_cluster_size)."""
+    cs = 4
+    while cs > 1 and (E % (4 * cs) != 0 or T < 8 * cs):
+        cs >>= 1
+    return 0 < T <= DOTATTN_MAX_T and 0 < D <= 512 and E > 0 and E % 4 == 0 and E // cs <= 1024
+
+
+class DotAttnMemStepFn(Function):
+    """One scaled dot-product attention step (src/module.py:189-212, one or more heads) on an attention memory:
+    forward = b200asr_dotattn_fwd (one launch); backward = b200asr_dotattn_bwd_acc (d(key) added into the memory, no
+    d(value) write; AttnMemFn forms d(value) once after the loop)."""
+
+    @staticmethod
+    def forward(ctx, mem, token, q, key, value, enc_len, num_head, temperature):
+        ctx.set_materialize_grads(False)
+        lib = L.load()
+        q = _f32c(q)
+        R, T, D = key.shape
+        E = value.shape[2]
+        dev = key.device
+        enc_len = enc_len.to(device=dev, dtype=torch.int64).contiguous()
+        attn = torch.empty((R, T), device=dev, dtype=torch.float32)
+        cvec = torch.empty((R, E), device=dev, dtype=torch.float32)
+        # algorithmic bytes: key + value read once, q / attn / ctx / lengths
+        with L.timed("dotattn_fwd", 4 * R * T * (D + E) + 4 * R * (D + T + E) + 8 * (R // num_head)):
+            L.check(lib.b200asr_dotattn_fwd(L.ptr(q), L.ptr(key), L.ptr(value), L.ptr(enc_len), int(num_head),
+                                            float(temperature), R, T, D, E, L.ptr(attn), L.ptr(cvec), L.stream()),
+                    "dotattn_fwd")
+        ctx.save_for_backward(q, key, value, enc_len, attn)
+        ctx.mem = mem
+        ctx.dims = (R, T, D, E, int(num_head))
+        ctx.temperature = float(temperature)
+        return cvec, attn
+
+    @staticmethod
+    def backward(ctx, dctx, dattn):
+        lib = L.load()
+        q, key, value, enc_len, attn = ctx.saved_tensors
+        R, T, D, E, N = ctx.dims
+        mem = ctx.mem
+        dev = key.device
+        CS = lib.b200asr_locattn_cluster_size(T, E)
+        if mem.dkey is None:
+            mem.dkey = torch.zeros((R, T, D), device=dev, dtype=torch.float32)
+        dctx = _f32c(dctx) if dctx is not None else torch.zeros((R, E), device=dev)
+        dattn = _f32c(dattn) if dattn is not None else None
+        dq_part = torch.empty((R, CS, D), device=dev, dtype=torch.float32)
+        # value read once, key read and d(key) read + written once; q, attn, dattn, dctx, dq partials, lengths
+        with L.timed("dotattn_bwd_acc", 4 * R * T * (2 * D + E) + 4 * R * (D + 2 * T + E + CS * D) + 8 * (R // N)):
+            L.check(lib.b200asr_dotattn_bwd_acc(L.ptr(q), L.ptr(key), L.ptr(value), L.ptr(enc_len), N, ctx.temperature,
+                                                L.ptr(attn), L.ptr(dctx), L.ptr(dattn), R, T, D, E, L.ptr(dq_part),
+                                                L.ptr(mem.dkey), L.stream()), "dotattn_bwd_acc")
+        mem.attn.append(attn)
+        mem.dctx.append(dctx)
+        token_grad = torch.zeros(1, device=dev, dtype=torch.float32)
+        return None, token_grad, dq_part.sum(1), None, None, None, None, None
+
+
+def dot_attention_mem_step(mem, token, q, key, value, enc_len, num_head, temperature):
+    """-> (context [R,E], attn [R,T]) with R = B * num_head rows; mem, key, value and token come from
+    attention_memory(key, value)."""
+    return DotAttnMemStepFn.apply(mem, token, q, key, value, enc_len, num_head, temperature)
 
 
 # ----------------------------------------------------------------------------------------------------------

@@ -205,6 +205,29 @@ B200ASR_API int b200asr_locattn_bwd_acc(const float* q, const float* key, const 
 B200ASR_API int b200asr_attn_dvalue(const float* attn_steps, const float* dctx_steps, int B, int L, int T, int E,
                                     float* dvalue, int accumulate, b200asr_stream stream);
 
+/* ---- K12d: scaled dot-product attention step, one or more heads, forward and decode-loop backward ----------------
+ * replaces src/module.py:198-212 (ScaleDotAttention.forward) + :189-195 (_attend), called from src/asr.py:307.  Rows are
+ * R = B * num_head (row r = b * num_head + n), row r masked by len = clamp(enc_len[r / num_head], 0, T):
+ *   q [R,D] (already tanh(proj_q(h)) per head), key [R,T,D], value [R,T,E] (the tensor Attention.forward forms,
+ *   including its value.repeat(num_head, 1, 1) without a value projection), enc_len [B] i64
+ *   ->  e[t] = (q . key[r,t]) / temperature for t < len;  attn [R,T] = softmax(e) over t < len, exactly 0 at t >= len;
+ *       ctx [R,E] = sum_t attn[t] value[r,t].
+ * backward (the decode loop's form, as b200asr_locattn_bwd_acc): dctx [R,E], dattn [R,T] or NULL;
+ *   g[t] = dctx . value[r,t] + dattn[t], de[t] = attn[t] (g[t] - sum attn g) / temperature  ->  dq_part [R,CS,D]
+ *   (sum over CS = dq), dkey_acc [R,T,D] += de[t] q for t < len.  No d(value): b200asr_attn_dvalue forms it once after the
+ *   loop from the stacked (attn_l, dctx_l).  Frames t >= len are never read and receive nothing.
+ * CS = b200asr_locattn_cluster_size(T, E) CTAs cooperate per row.  Limits (b200asr_dotattn_supported): 0 < T <=
+ * B200ASR_DOTATTN_MAX_T, D <= 512, E % 4 == 0, E / CS <= 1024.  Deterministic: no float atomics.                 */
+#define B200ASR_DOTATTN_MAX_T 8192
+B200ASR_API int b200asr_dotattn_supported(int T, int D, int E);
+B200ASR_API int b200asr_dotattn_fwd(const float* q, const float* key, const float* value, const long long* enc_len,
+                                    int num_head, float temperature, int R, int T, int D, int E, float* attn, float* ctx,
+                                    b200asr_stream stream);
+B200ASR_API int b200asr_dotattn_bwd_acc(const float* q, const float* key, const float* value, const long long* enc_len,
+                                        int num_head, float temperature, const float* attn, const float* dctx,
+                                        const float* dattn, int R, int T, int D, int E, float* dq_part, float* dkey_acc,
+                                        b200asr_stream stream);
+
 /* ---- K15: cross-entropy (log-softmax + NLL, ignore_index) forward + logit gradient ----------------------
  * replaces torch.nn.CrossEntropyLoss(ignore_index=0) at bin/train_asr.py:47,127-131.  row_loss [n_rows] =
  * lse(x) - x[target] (0 for ignored rows); dlogits (optional) = grad_scale[0] * (softmax(x) - onehot), zero rows
