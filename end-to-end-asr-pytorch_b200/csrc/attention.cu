@@ -66,7 +66,8 @@ __device__ __forceinline__ void energy_to_cluster(cg::cluster_group& cluster, fl
     }
 }
 
-// masked softmax over the full time axis (redundantly in every CTA; masked frames hold -inf and get exactly 0):
+// masked softmax over the full time axis (redundantly in every CTA; masked frames hold -inf and get exactly 0; a row
+// with len 0 gets 0/0 = NaN everywhere, as the reference's softmax of an all -inf row):
 // s_energy becomes the attention; attn_row (one CTA of the cluster) receives a copy
 __device__ __forceinline__ void softmax_in_place(float* s_energy, float* s_scratch, int T, float* attn_row) {
     float mx = NEG_INF;
@@ -119,6 +120,7 @@ __device__ __forceinline__ void context_slice(const AttnParams& p, int b, int ra
                 const float4 o = *reinterpret_cast<const float4*>(s_ctx + (size_t)(g * cpp + col - cbase) * 4);
                 acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w;
             }
+            if (len == 0) acc = make_float4(NAN, NAN, NAN, NAN);   // the reference's 0/0 attention reaches the context
             *reinterpret_cast<float4*>(p.ctx + (size_t)b * E + (size_t)rank * ES + col * 4) = acc;
         }
         __syncthreads();
@@ -167,7 +169,7 @@ __device__ __forceinline__ void dattn_partials(const AttnParams& p, cg::cluster_
                 if (t < len) part += dc.x * v.x + dc.y * v.y + dc.z * v.z + dc.w * v.w;
                 if (p.dvalue) {
                     float4 dv = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (t < len) dv = make_float4(a * dc.x, a * dc.y, a * dc.z, a * dc.w);
+                    if (t < len || len == 0) dv = make_float4(a * dc.x, a * dc.y, a * dc.z, a * dc.w);   // len 0: NaN
                     *reinterpret_cast<float4*>(dvr + e) = dv;
                 }
             }
@@ -568,16 +570,20 @@ __global__ void __launch_bounds__(MINB == 2 ? 384 : 512, MINB) dotattn_bwd_kerne
     }
 }
 
+// CTAs per row: 4 where the feature split allows it (E % (4 CS) == 0); fewer for short memories (T < 8 CS: a speed
+// preference only), but never so few that E / CS exceeds the backward's 1024-column limit.
 static int pick_cluster(int T, int E) {
     int cs = 4;
-    while (cs > 1 && (E % (4 * cs) != 0 || T < 8 * cs)) cs >>= 1;
+    while (cs > 1 && (E % (4 * cs) != 0 || (T < 8 * cs && E / (cs / 2) <= 1024))) cs >>= 1;
     return cs;
 }
 
+constexpr size_t ATT_STATIC_SMEM = 32 * sizeof(float);   // s_scratch of every attention kernel
+
 static int launch_attn(const char* what, const void* fn, AttnParams& p, int threads, size_t smem,
                        cudaStream_t stream) {
-    B200_REQUIRE(smem <= (size_t)max_optin_smem(), "%s: %zu bytes of shared memory needed (T=%d D=%d too large)", what,
-                 smem, p.T, p.D);
+    B200_REQUIRE(smem + ATT_STATIC_SMEM <= (size_t)max_optin_smem(),
+                 "%s: %zu bytes of shared memory needed (T=%d D=%d too large)", what, smem + ATT_STATIC_SMEM, p.T, p.D);
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(p.B * p.CS);

@@ -1251,7 +1251,7 @@ DOTATTN_MAX_T = 8192          # B200ASR_DOTATTN_MAX_T of include/b200asr.h
 def dot_attention_supported(T, D, E):
     """The limits of b200asr_dotattn_fwd / _bwd_acc (include/b200asr.h; cluster rule of b200asr_locattn_cluster_size)."""
     cs = 4
-    while cs > 1 and (E % (4 * cs) != 0 or T < 8 * cs):
+    while cs > 1 and (E % (4 * cs) != 0 or (T < 8 * cs and E // (cs // 2) <= 1024)):
         cs >>= 1
     return 0 < T <= DOTATTN_MAX_T and 0 < D <= 512 and E > 0 and E % 4 == 0 and E // cs <= 1024
 

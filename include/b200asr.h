@@ -180,7 +180,9 @@ B200ASR_API int b200asr_gru_cell_bwd(const float* gates, const float* h_prev, co
  * backward: dctx [B,E], dattn [B,T] or NULL -> dq_part [B,CS,D] (sum over CS = dq), dkey [B,T,D], dvalue [B,T,E],
  * dprev [B,T], wpart [B*CS, P] with P = D*K + K*(2R+1) + D + 1 laid out (d w_proj | d w_conv | d w_energy | d b_energy);
  * the caller sums wpart over its first axis.  CS = b200asr_locattn_cluster_size(T, E) CTAs cooperate per utterance
- * through distributed shared memory.  K <= 16, E % 4 == 0, D <= 512, E / CS <= 1024.                                              */
+ * through distributed shared memory.  K <= 16, E % 4 == 0, D <= 512, E / CS <= 1024 (the cluster rule keeps E / CS
+ * <= 1024 for every T whenever E % 16 == 0 and E <= 4096).  An utterance with enc_len 0 gets the reference's masked
+ * softmax of no frames: NaN attention, NaN context and NaN d(value); its other gradients are 0.                   */
 B200ASR_API int b200asr_locattn_cluster_size(int T, int E);
 B200ASR_API size_t b200asr_locattn_wpart_floats(int D, int K, int R);
 B200ASR_API int b200asr_locattn_fwd(const float* q, const float* key, const float* value, const float* prev_att,

@@ -48,7 +48,9 @@ def test_null_pointers_and_bad_sizes_are_refused(pkg, which):
         assert err.startswith(name + ":") and msg in err, (args, err)
 
 
-def test_python_limits_agree_with_the_library(pkg):
+def test_python_limits_follow_the_library_cluster_rule(pkg):
+    """dot_attention_supported equals b200asr_dotattn_supported over a sweep of shapes; a short memory keeps as many
+    CTAs as E / CS <= 1024 needs, and only a width the feature split cannot divide is refused."""
     lib = pkg.load_library()
     assert pkg.ops.DOTATTN_MAX_T == 8192
     Ts = [1, 7, 8, 15, 16, 31, 32, 149, 4096, 8191, 8192, 8193]
@@ -63,7 +65,8 @@ def test_python_limits_agree_with_the_library(pkg):
                     assert _fwd(lib, [FAKE] * 6, 1, 2, T, D, E) == -1, (T, D, E)
                     assert _bwd(lib, [FAKE] * 8, 1, 2, T, D, E) == -1, (T, D, E)
     assert pkg.ops.dot_attention_supported(4096, 512, 4096)     # 40 s without time reduction, the widest rows
-    assert not pkg.ops.dot_attention_supported(8, 16, 2048)      # a short memory gets a 1-CTA cluster: E / CS > 1024
+    assert pkg.ops.dot_attention_supported(8, 16, 2048)          # a short memory keeps a 2-CTA cluster: E / CS = 1024
+    assert not pkg.ops.dot_attention_supported(8, 16, 4100)      # E % 8 != 0 leaves one CTA: E / CS > 1024
 
 
 @pytest.mark.parametrize("kind", ["dot1", "dotrep"])
