@@ -765,3 +765,366 @@ extern "C" int b200asr_dotattn_bwd_acc(const float* q, const float* key, const f
     return launch_attn("dotattn_bwd_acc", two_per_sm ? (const void*)dotattn_bwd_kernel<2> : (const void*)dotattn_bwd_kernel<1>,
                        p, threads, smem, (cudaStream_t)stream);
 }
+
+// ---- multi-head location-aware attention ---------------------------------------------------------------------------
+// The reference's LocationAwareAttention with N > 1 heads (src/module.py:234-258): ONE location convolution per
+// utterance over the N channels of prev_att [B,N,T], its projection shared by the N heads (loc.repeat(1,N,1,1)); row
+// r = b*N + n of q / key / value / attn / ctx is head n of utterance b, masked by len[b]:
+//   conv[k,t]  = sum_n sum_j w_conv[k,n,j] * prev[b,n,t+j-R]         (one fmaf chain, n outer, j inner)
+//   loc[t,d]   = tanh(sum_k w_proj[d,k] * conv[k,t])
+//   e[r,t]     = (b_e + sum_d w_e[d] * tanh(key[r,t,d] + q[r,d] + loc[t,d])) / temperature
+// One cluster of CS CTAs per UTTERANCE covers all N heads: the CTAs split time for conv / loc / the N heads' energies
+// (conv and loc computed once per frame, not once per head), exchange the N energy rows through distributed shared
+// memory, and each runs the N masked softmaxes and an E/CS slice of the N contexts.  The backward sums d(loc) over the
+// heads in shared memory in head order (no atomics) and writes d(prev) for all N channels.
+namespace b200asr {
+
+constexpr int LH_TT = 16;  // frame tile of the multi-head backward
+
+// conv[k][tl] over the N channels for frames [t0, t0+nts) into s_conv[k*stride + tl]; s_prev holds N rows of T + 2R
+__device__ __forceinline__ void conv_heads_slice(const float* s_prev, const float* s_w, float* s_conv, int K, int N,
+                                                 int W, int TP, int t0, int nts, int stride) {
+    for (int idx = threadIdx.x; idx < K * nts; idx += blockDim.x) {
+        const int k = idx / nts, tl = idx - k * nts;
+        float acc = 0.f;
+        for (int n = 0; n < N; ++n) {
+            const float* pw = s_w + (k * N + n) * W;
+            const float* pp = s_prev + n * TP + t0 + tl;
+            for (int j = 0; j < W; ++j) acc = fmaf(pw[j], pp[j], acc);
+        }
+        s_conv[k * stride + tl] = acc;
+    }
+}
+
+// prev rows of utterance b (zero halo of R frames each side), the weights and the N query rows into shared memory
+__device__ __forceinline__ void heads_load_common(const AttnParams& p, int b, float* s_prev, float* s_w, float* s_pw,
+                                                  float* s_ew, float* s_q) {
+    const int N = p.N, T = p.T, D = p.D, K = p.K, R = p.R, W = 2 * R + 1, TP = T + 2 * R;
+    for (int i = threadIdx.x; i < N * TP; i += blockDim.x) {
+        const int n = i / TP, t = i - n * TP - R;
+        s_prev[i] = (t >= 0 && t < T) ? p.prev[((size_t)b * N + n) * T + t] : 0.f;
+    }
+    for (int i = threadIdx.x; i < K * N * W; i += blockDim.x) s_w[i] = p.w_conv[i];
+    for (int i = threadIdx.x; i < D * K; i += blockDim.x) s_pw[i] = p.w_proj[i];
+    for (int i = threadIdx.x; i < D; i += blockDim.x) s_ew[i] = p.w_e[i];
+    for (int i = threadIdx.x; i < N * D; i += blockDim.x) s_q[i] = p.q[(size_t)b * N * D + i];
+}
+
+__global__ void __launch_bounds__(512, 1) locattn_heads_fwd_kernel(AttnParams p) {
+    extern __shared__ __align__(16) float sm[];
+    __shared__ float s_scratch[32];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int CS = p.CS;
+    const int rank = (int)cluster.block_rank();
+    const int b = blockIdx.x / CS;                  // utterance
+    const int N = p.N, T = p.T, D = p.D, K = p.K, R = p.R, W = 2 * R + 1, TP = T + 2 * R;
+    const int TS = (T + CS - 1) / CS;
+    float* s_prev = sm;                             // [N*(T + 2R)]
+    float* s_w = s_prev + N * TP;                   // [K*N*W]
+    float* s_pw = s_w + K * N * W;                  // [D*K]
+    float* s_ew = s_pw + D * K;                     // [D]
+    float* s_q = s_ew + D;                          // [N*D]
+    float* s_energy = s_q + N * D;                  // [N*T]
+    float* s_conv = s_energy + N * T;               // [K*TS]
+    float* s_ctx = sm + (((s_conv + K * TS) - sm + 3) & ~3);   // [blockDim.x * 4] partial sums, 16-B aligned
+
+    const int len = clampi((int)p.len[b], 0, T);
+    heads_load_common(p, b, s_prev, s_w, s_pw, s_ew, s_q);
+    cluster.sync();  // all CTAs of the cluster are running (required before any remote shared-memory access)
+
+    const int t0 = rank * TS;
+    const int nts = max(0, min(min(T, t0 + TS), len) - t0);
+    conv_heads_slice(s_prev, s_w, s_conv, K, N, W, TP, t0, nts, TS);
+    __syncthreads();
+
+    // one warp per frame of my slice: loc once, then the N heads' energies -> every CTA of the cluster
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    const float be = p.b_e[0];
+    for (int tl = warp; tl < TS; tl += nw) {
+        const int t = t0 + tl;
+        if (t >= T) break;
+        if (t >= len) {
+            if (lane == 0)
+                for (int n = 0; n < N; ++n) energy_to_cluster(cluster, s_energy + n * T, rank, CS, t, NEG_INF);
+            continue;
+        }
+        float lc[16];                                   // loc[t, lane + 32 i] (D <= 512)
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const int d = lane + 32 * i;
+            lc[i] = 0.f;
+            if (d < D) {
+                float pre = 0.f;
+                for (int k = 0; k < K; ++k) pre = fmaf(s_pw[d * K + k], s_conv[k * TS + tl], pre);
+                lc[i] = tanhf(pre);
+            }
+        }
+        for (int n = 0; n < N; ++n) {
+            const float* kr = p.key + (((size_t)b * N + n) * T + t) * D;
+            float kv[16];                               // the frame's key row of head n, all loads in flight at once
+#pragma unroll
+            for (int i = 0; i < 16; ++i) kv[i] = (lane + 32 * i < D) ? kr[lane + 32 * i] : 0.f;
+            float part = 0.f;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                const int d = lane + 32 * i;
+                if (d < D) part = fmaf(s_ew[d], tanhf(kv[i] + s_q[n * D + d] + lc[i]), part);
+            }
+            const float e = warp_sum(part) + be;        // divided by the temperature below
+            if (lane == 0) energy_to_cluster(cluster, s_energy + n * T, rank, CS, t, e);
+        }
+    }
+    cluster.sync();  // the last remote access of this kernel: no peer touches this CTA's shared memory after it
+    // the division outside the energy loop: its slow path is a subroutine call, which there would need a stack frame
+    for (int i = threadIdx.x; i < N * T; i += blockDim.x) s_energy[i] = s_energy[i] / p.temperature;
+    __syncthreads();
+
+#pragma unroll 1
+    for (int n = 0; n < N; ++n) {
+        const int r = b * N + n;
+        softmax_in_place(s_energy + n * T, s_scratch, T, rank == 0 ? p.attn + (size_t)r * T : nullptr);
+        context_slice(p, r, rank, len, s_energy + n * T, s_ctx);
+    }
+}
+
+// Backward of one decode step on the per-batch accumulators (the decode loop's form): per head the d(attn) partials
+// and the softmax backward of the shared helpers; then, in tiles of LH_TT frames of my time slice, one thread per
+// attention dim recomputes conv / loc once per frame and, per head, s = tanh(key + q + loc): d(key) += dpre,
+// d(q) and d(w_e) partials, and the head sum dpre_0 + ... + dpre_{N-1} in s_dloc (head order) before d(loc) =
+// sum * (1 - loc^2) feeds d(w_proj) and d(conv).  d(conv) goes to every peer's full-time buffer; each CTA then forms
+// its slice of d(w_conv) [K,N,W] and d(prev) [N, slice].  MINB as in the single-head backward.
+template <int MINB>
+__global__ void __launch_bounds__(MINB == 2 ? 384 : 512, MINB) locattn_heads_bwd_kernel(AttnParams p) {
+    extern __shared__ __align__(16) float sm[];
+    __shared__ float s_scratch[32];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int CS = p.CS;
+    const int rank = (int)cluster.block_rank();
+    const int b = blockIdx.x / CS;
+    const int N = p.N, T = p.T, D = p.D, K = p.K, R = p.R, W = 2 * R + 1, TP = T + 2 * R;
+    const int TS = (T + CS - 1) / CS;
+    float* s_prev = sm;                             // [N*(T + 2R)]
+    float* s_w = s_prev + N * TP;                   // [K*N*W]
+    float* s_pw = s_w + K * N * W;                  // [D*K]
+    float* s_ew = s_pw + D * K;                     // [D]
+    float* s_q = s_ew + D;                          // [N*D]
+    float* s_attn = s_q + N * D;                    // [N*T]
+    float* s_de = s_attn + N * T;                   // [N*T]
+    float* s_part = s_de + N * T;                   // [N*CS*T] partial d(attn) of every peer, per head
+    float* s_conv = s_part + N * CS * T;            // [K*LH_TT]
+    float* s_loc = s_conv + K * LH_TT;              // [LH_TT*D]
+    float* s_dloc = s_loc + LH_TT * D;              // [LH_TT*D]
+    float* s_dq = s_dloc + LH_TT * D;               // [N*D]    d(q) of my slice, thread d owns column d
+    float* s_dpw = s_dq + N * D;                    // [D*K]    d(w_proj) of my slice, thread d owns row d
+    float* s_dconv = s_dpw + D * K;                 // [K*(T + 2R)] full-time d(conv) with zero halo
+
+    const int len = clampi((int)p.len[b], 0, T);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    heads_load_common(p, b, s_prev, s_w, s_pw, s_ew, s_q);
+    for (int i = threadIdx.x; i < N * T; i += blockDim.x) s_attn[i] = p.attn_in[(size_t)b * N * T + i];
+    for (int i = threadIdx.x; i < N * D; i += blockDim.x) s_dq[i] = 0.f;
+    for (int i = threadIdx.x; i < D * K; i += blockDim.x) s_dpw[i] = 0.f;
+    for (int i = threadIdx.x; i < K * TP; i += blockDim.x) s_dconv[i] = 0.f;
+    cluster.sync();  // all CTAs running + local init visible before any remote shared-memory access
+
+    // A. d(attn) partials of the N rows over my feature slice
+#pragma unroll 1
+    for (int n = 0; n < N; ++n)
+        dattn_partials<MINB == 2 ? 4 : 8>(p, cluster, b * N + n, rank, len, s_attn + n * T, s_part + n * CS * T);
+    cluster.sync();
+    // B. softmax backward of the N rows (every CTA, full time axis)
+#pragma unroll 1
+    for (int n = 0; n < N; ++n)
+        softmax_bwd(p, b * N + n, len, s_attn + n * T, s_part + n * CS * T, s_de + n * T, s_scratch);
+
+    // C. my time slice, frames t < len only
+    const int t0s = rank * TS;
+    const int t1s = min(T, t0s + TS);
+    const int tend = min(t1s, len);
+    const int d_own = threadIdx.x;  // one thread per attention dim (blockDim >= D)
+    float dew_acc = 0.f, deb_acc = 0.f;
+    for (int tb = t0s; tb < tend; tb += LH_TT) {
+        const int tv = min(tend - tb, LH_TT);
+        conv_heads_slice(s_prev, s_w, s_conv, K, N, W, TP, tb, tv, LH_TT);
+        __syncthreads();
+        if (d_own < D) {
+            for (int tl = 0; tl < tv; ++tl) {
+                float pre = 0.f;
+                for (int k = 0; k < K; ++k) pre = fmaf(s_pw[d_own * K + k], s_conv[k * LH_TT + tl], pre);
+                s_loc[tl * D + d_own] = tanhf(pre);
+                s_dloc[tl * D + d_own] = 0.f;
+            }
+            const float ew = s_ew[d_own];
+            for (int n = 0; n < N; ++n) {
+                const size_t off = (((size_t)b * N + n) * T + tb) * D + d_own;
+                const float qd = s_q[n * D + d_own];
+                const float* de_n = s_de + n * T + tb;
+                float dq = 0.f;
+#pragma unroll 2                                    // 4 spills in the two-CTAs-per-SM instance
+                for (int tl = 0; tl < tv; ++tl) {
+                    const float s = tanhf(p.key[off + (size_t)tl * D] + qd + s_loc[tl * D + d_own]);
+                    const float de = de_n[tl];
+                    const float dpre = de * ew * (1.f - s * s);
+                    dew_acc = fmaf(de, s, dew_acc);
+                    dq += dpre;
+                    p.dkey[off + (size_t)tl * D] += dpre;
+                    s_dloc[tl * D + d_own] += dpre;
+                }
+                s_dq[n * D + d_own] += dq;
+            }
+            for (int tl = 0; tl < tv; ++tl) {
+                const float loc = s_loc[tl * D + d_own];
+                const float dloc = s_dloc[tl * D + d_own] * (1.f - loc * loc);
+                s_dloc[tl * D + d_own] = dloc;
+                for (int k = 0; k < K; ++k)
+                    s_dpw[d_own * K + k] = fmaf(dloc, s_conv[k * LH_TT + tl], s_dpw[d_own * K + k]);
+            }
+        }
+        if (threadIdx.x == 0)
+            for (int n = 0; n < N; ++n)
+                for (int tl = 0; tl < tv; ++tl) deb_acc += s_de[n * T + tb + tl];
+        __syncthreads();
+        // d(conv)[k][t] = sum_d dloc[t,d] * w_proj[d,k]  -> every peer's full-time buffer
+        for (int idx = warp; idx < tv * K; idx += nw) {
+            const int tl = idx / K, k = idx - tl * K;
+            float part = 0.f;
+            for (int d = lane; d < D; d += 32) part = fmaf(s_dloc[tl * D + d], s_pw[d * K + k], part);
+            part = warp_sum(part);
+            if (lane == 0) {
+                for (int rr = 0; rr < CS; ++rr) {
+                    float* dst = (rr == rank) ? s_dconv : cluster.map_shared_rank(s_dconv, rr);
+                    dst[k * TP + R + tb + tl] = part;
+                }
+            }
+        }
+        __syncthreads();
+    }
+    cluster.sync();  // the last remote access of this kernel: every peer's d(conv) is in place
+
+    // D. d(w_conv)[k,n,j] partial over my slice, d(prev)[n, t'] for my slice
+    const int P = D * K + K * N * W + D + 1;
+    float* wp = p.wpart + (size_t)(b * CS + rank) * P;
+    const int tv_all = max(0, tend - t0s);
+    for (int idx = threadIdx.x; idx < K * N * W; idx += blockDim.x) {
+        const int k = idx / (N * W), nj = idx - k * N * W, n = nj / W, j = nj - n * W;
+        const float* dc = s_dconv + k * TP + R + t0s;
+        const float* pp = s_prev + n * TP + t0s + j;
+        float acc = 0.f;
+        for (int tl = 0; tl < tv_all; ++tl) acc = fmaf(dc[tl], pp[tl], acc);
+        wp[D * K + idx] += acc;
+    }
+    // dprev[n, t'] = sum_k sum_j dconv[k][t' - j + R] * w[k,n,j]   (dconv zero outside [0, len))
+    const int ns = t1s - t0s;
+    for (int o = warp; o < N * ns; o += nw) {
+        const int n = o / ns, tp = t0s + (o - n * ns);
+        float part = 0.f;
+        for (int idx = lane; idx < K * W; idx += 32) {
+            const int k = idx / W, j = idx - k * W;
+            part = fmaf(s_dconv[k * TP + R + tp - j + R], s_w[(k * N + n) * W + j], part);
+        }
+        part = warp_sum(part);
+        if (lane == 0) p.dprev[((size_t)b * N + n) * T + tp] = part;
+    }
+    // E. per-CTA partial weight gradients and d(q)
+    if (d_own < D) {
+        for (int k = 0; k < K; ++k) wp[d_own * K + k] += s_dpw[d_own * K + k];
+        wp[D * K + K * N * W + d_own] += dew_acc;
+        for (int n = 0; n < N; ++n) p.dq_part[(((size_t)b * N + n) * CS + rank) * D + d_own] = s_dq[n * D + d_own];
+    }
+    if (threadIdx.x == 0) wp[D * K + K * N * W + D] += deb_acc;
+}
+
+static size_t locattn_heads_fwd_smem(int N, int T, int D, int K, int R, int CS) {
+    const size_t W = 2 * (size_t)R + 1, TP = (size_t)T + 2 * R, TS = ((size_t)T + CS - 1) / CS;
+    const size_t head = N * TP + K * N * W + (size_t)D * K + D + (size_t)N * D + (size_t)N * T + K * TS;
+    return sizeof(float) * ((head + 3) / 4 * 4 + 512 * 4);
+}
+
+static size_t locattn_heads_bwd_smem(int N, int T, int D, int K, int R, int CS) {
+    const size_t W = 2 * (size_t)R + 1, TP = (size_t)T + 2 * R;
+    return sizeof(float) * (N * TP + K * N * W + 2 * (size_t)D * K + D + 2 * (size_t)N * D + 2 * (size_t)N * T +
+                            (size_t)N * CS * T + (size_t)K * LH_TT + 2 * (size_t)LH_TT * D + K * TP);
+}
+
+// The limits of include/b200asr.h, checked before any CUDA call (b200asr_locattn_heads_supported reports the same set;
+// ops.loc_attention_heads_supported restates it).
+static int locattn_heads_check(const char* what, int B, int N, int T, int D, int E, int K, int R) {
+    B200_REQUIRE(B > 0 && N > 0 && T > 0 && D > 0 && E > 0 && K > 0 && R >= 0,
+                 "%s: bad sizes B=%d N=%d T=%d D=%d E=%d K=%d R=%d", what, B, N, T, D, E, K, R);
+    B200_REQUIRE(N <= 16, "%s: at most 16 heads (got %d)", what, N);
+    B200_REQUIRE(K <= 16, "%s: at most 16 location kernels (got %d)", what, K);
+    B200_REQUIRE(D <= 512, "%s: attention dim %d > 512", what, D);
+    B200_REQUIRE(E % 4 == 0, "%s: value dim %d must be a multiple of 4", what, E);
+    const int cs = pick_cluster(T, E);
+    B200_REQUIRE(E / cs <= 1024, "%s: value dim %d too large for %d-CTA clusters", what, E, cs);
+    const size_t fwd = locattn_heads_fwd_smem(N, T, D, K, R, cs), bwd = locattn_heads_bwd_smem(N, T, D, K, R, cs);
+    const size_t need = fwd > bwd ? fwd : bwd;
+    B200_REQUIRE(need + ATT_STATIC_SMEM <= (size_t)max_optin_smem(),
+                 "%s: %zu bytes of shared memory needed (N=%d T=%d D=%d K=%d R=%d too large)", what,
+                 need + ATT_STATIC_SMEM, N, T, D, K, R);
+    return B200_OK;
+}
+
+static AttnParams locattn_heads_params(const float* q, const float* key, const float* value, const float* prev_att,
+                                       const long long* enc_len, const float* w_conv, const float* w_proj,
+                                       const float* w_energy, float temperature, int B, int N, int T, int D, int E,
+                                       int K, int R) {
+    AttnParams p = {};
+    p.q = q; p.key = key; p.value = value; p.prev = prev_att; p.len = enc_len; p.w_conv = w_conv; p.w_proj = w_proj;
+    p.w_e = w_energy; p.temperature = temperature; p.B = B; p.N = N; p.T = T; p.D = D; p.E = E; p.K = K; p.R = R;
+    p.CS = pick_cluster(T, E);
+    return p;
+}
+
+}  // namespace b200asr
+
+extern "C" int b200asr_locattn_heads_supported(int N, int T, int D, int E, int K, int R) {
+    return locattn_heads_check("locattn_heads_supported", 1, N, T, D, E, K, R) == B200_OK;
+}
+
+extern "C" size_t b200asr_locattn_heads_wpart_floats(int N, int D, int K, int R) {
+    return (size_t)D * K + (size_t)K * N * (2 * R + 1) + D + 1;
+}
+
+extern "C" int b200asr_debug_locattn_heads_bwd_minb(int B, int N, int T, int D, int E) {
+    return (B > 0 && N > 0 && T > 0 && E > 0) ? locattn_bwd_minb(B, T, D, E) : 0;   // the single-head rule
+}
+
+extern "C" int b200asr_locattn_heads_fwd(const float* q, const float* key, const float* value, const float* prev_att,
+                                         const long long* enc_len, const float* w_conv, const float* w_proj,
+                                         const float* w_energy, const float* b_energy, float temperature, int B,
+                                         int N, int T, int D, int E, int K, int R, float* attn, float* ctx,
+                                         b200asr_stream stream) {
+    B200_REQUIRE(q && key && value && prev_att && enc_len && w_conv && w_proj && w_energy && b_energy && attn && ctx,
+                 "locattn_heads_fwd: null pointer");
+    const int rc = locattn_heads_check("locattn_heads_fwd", B, N, T, D, E, K, R);
+    if (rc != B200_OK) return rc;
+    AttnParams p = locattn_heads_params(q, key, value, prev_att, enc_len, w_conv, w_proj, w_energy, temperature, B, N,
+                                        T, D, E, K, R);
+    p.b_e = b_energy; p.attn = attn; p.ctx = ctx;
+    return launch_attn("locattn_heads_fwd", (const void*)locattn_heads_fwd_kernel, p, 512,
+                       locattn_heads_fwd_smem(N, T, D, K, R, p.CS), (cudaStream_t)stream);
+}
+
+extern "C" int b200asr_locattn_heads_bwd_acc(const float* q, const float* key, const float* value,
+                                             const float* prev_att, const long long* enc_len, const float* w_conv,
+                                             const float* w_proj, const float* w_energy, float temperature,
+                                             const float* attn, const float* dctx, const float* dattn, int B, int N,
+                                             int T, int D, int E, int K, int R, float* dq_part, float* dkey_acc,
+                                             float* dprev, float* wpart_acc, b200asr_stream stream) {
+    B200_REQUIRE(q && key && value && prev_att && enc_len && w_conv && w_proj && w_energy && attn && dctx && dq_part &&
+                     dkey_acc && dprev && wpart_acc,
+                 "locattn_heads_bwd_acc: null pointer");
+    const int rc = locattn_heads_check("locattn_heads_bwd_acc", B, N, T, D, E, K, R);
+    if (rc != B200_OK) return rc;
+    AttnParams p = locattn_heads_params(q, key, value, prev_att, enc_len, w_conv, w_proj, w_energy, temperature, B, N,
+                                        T, D, E, K, R);
+    p.attn_in = attn; p.dctx = dctx; p.dattn = dattn; p.dq_part = dq_part; p.dkey = dkey_acc; p.dprev = dprev;
+    p.wpart = wpart_acc; p.accumulate = 1;
+    int threads = (D + 31) / 32 * 32;
+    if (threads < 128) threads = 128;
+    const bool two_per_sm = locattn_bwd_minb(B, T, D, E) == 2;
+    return launch_attn("locattn_heads_bwd_acc",
+                       two_per_sm ? (const void*)locattn_heads_bwd_kernel<2> : (const void*)locattn_heads_bwd_kernel<1>,
+                       p, threads, locattn_heads_bwd_smem(N, T, D, K, R, p.CS), (cudaStream_t)stream);
+}

@@ -52,6 +52,7 @@ SIGNATURES = {
     "b200asr_debug_ctc_variant": (c_int, [c_int]),
     "b200asr_debug_locattn_bwd_minb": (c_int, [c_int, c_int, c_int, c_int]),
     "b200asr_debug_dotattn_bwd_minb": (c_int, [c_int, c_int, c_int]),
+    "b200asr_debug_locattn_heads_bwd_minb": (c_int, [c_int, c_int, c_int, c_int, c_int]),
     "b200asr_debug_gemm_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_size_t, POINTER(c_int)]),
     "b200asr_lstm_cell_fwd": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, _P]),
     "b200asr_lstm_cell_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P]),
@@ -70,6 +71,12 @@ SIGNATURES = {
     "b200asr_dotattn_fwd": (c_int, [_P, _P, _P, _P, c_int, c_float, c_int, c_int, c_int, c_int, _P, _P, _P]),
     "b200asr_dotattn_bwd_acc": (c_int, [_P, _P, _P, _P, c_int, c_float, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P,
                                         _P]),
+    "b200asr_locattn_heads_supported": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    "b200asr_locattn_heads_wpart_floats": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "b200asr_locattn_heads_fwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_float, c_int, c_int, c_int, c_int, c_int,
+                                          c_int, c_int, _P, _P, _P]),
+    "b200asr_locattn_heads_bwd_acc": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_float, _P, _P, _P, c_int, c_int, c_int,
+                                              c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     "b200asr_ce_fwd_bwd": (c_int, [_P, _P, c_longlong, c_longlong, c_int, _P, _P, _P, _P]),
     "b200asr_embedding_bwd_workspace_bytes": (c_size_t, [c_int, c_int]),
     "b200asr_embedding_bwd": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_size_t, _P]),

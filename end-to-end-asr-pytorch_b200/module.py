@@ -3,7 +3,8 @@
 
   RNNLayer               -> persistent BiLSTM kernels (ops.bilstm) + f16x3 input/weight-grad GEMMs (csrc/gemm.cu;
                             the cuBLAS 3xTF32 composition when the input width is not a multiple of 4)
-  LocationAwareAttention -> fused single-launch attention step (ops.loc_attention_step)
+  LocationAwareAttention -> fused single-launch attention step, one or more heads (ops.loc_attention_mem_step,
+                            ops.loc_attention_heads_mem_step; the library ops for CPU tensors and unsupported shapes)
   CNNExtractor           -> its Conv1d(k 4, s 2) on the 3xTF32 GEMM kernel (ops.conv1d_k4s2p1)
   VGGExtractor           -> its 3x3 convolutions as implicit GEMMs on the 3xTF32 kernel, ReLU and max-pool fused
                             (ops.vgg_extractor; the library sequence only for CPU tensors)
@@ -197,7 +198,8 @@ class ScaleDotAttention(BaseAttention):
 class LocationAwareAttention(BaseAttention):
     """Location-aware attention (src/module.py:215-258).  With one head (every BASELINE config) the whole step -
     conv over the previous alignment, location projection, energy, masked softmax, context - is ONE kernel launch
-    (ops.loc_attention_step); multi-head falls back to the unfused library ops."""
+    (ops.loc_attention_step); with N > 1 heads it is one launch too, one location convolution per utterance shared by
+    its heads (ops.loc_attention_heads_mem_step).  The library ops remain for CPU tensors and unsupported shapes."""
 
     def __init__(self, kernel_size, kernel_num, dim, num_head, temperature):
         super().__init__(temperature, num_head)
@@ -237,6 +239,16 @@ class LocationAwareAttention(BaseAttention):
             output, attn = ops.loc_attention_mem_step(mem, token, q, mk, mv, self.prev_att.view(bs, ts), self.k_len,
                                                       cw, pw, ew, eb, self.temperature)
             attn = attn.view(bs, 1, ts)
+        elif k.is_cuda and ops.loc_attention_heads_supported(self.num_head, ts, self.dim, v.shape[2],
+                                                             self.loc_conv.weight.shape[0],
+                                                             (self.loc_conv.weight.shape[2] - 1) // 2):
+            if self._mem is None:
+                self._mem = ops.attention_memory(k, v, self.loc_conv.weight, self.loc_proj.weight,
+                                                 self.gen_energy.weight, self.gen_energy.bias)
+            mem, mk, mv, cw, pw, ew, eb, token = self._mem
+            output, attn = ops.loc_attention_heads_mem_step(mem, token, q, mk, mv, self.prev_att, self.k_len,
+                                                            self.num_head, cw, pw, ew, eb, self.temperature)
+            attn = attn.view(bs, self.num_head, ts)
         else:
             loc = torch.tanh(self.loc_proj(self.loc_conv(self.prev_att).transpose(1, 2)))
             loc = loc.unsqueeze(1).repeat(1, self.num_head, 1, 1).view(-1, ts, self.dim)

@@ -1162,10 +1162,11 @@ class AttnMemFn(Function):
         d_loc = (None,) * len(g_loc)
         if mem.wpart is not None:
             s_conv, s_proj, s_ew, s_eb = ctx.shapes[2:]
-            K, _, W = s_conv
+            K, N, W = s_conv                                # conv weight [K, N, 2R+1]: N location channels (heads)
+            C = K * N * W
             wsum = mem.wpart.sum(0)
-            d_loc = (wsum[D * K:D * K + K * W].view(s_conv), wsum[:D * K].view(s_proj),
-                     wsum[D * K + K * W:D * K + K * W + D].view(s_ew), wsum[D * K + K * W + D:].view(s_eb))
+            d_loc = (wsum[D * K:D * K + C].view(s_conv), wsum[:D * K].view(s_proj),
+                     wsum[D * K + C:D * K + C + D].view(s_ew), wsum[D * K + C + D:].view(s_eb))
         add = lambda a, b: a if b is None else (b if a is None else a + b)
         mem.dkey = mem.wpart = None
         mem.attn, mem.dctx = [], []
@@ -1173,8 +1174,8 @@ class AttnMemFn(Function):
 
 
 def attention_memory(key, value, conv_w=None, proj_w=None, e_w=None, e_b=None):
-    """-> (mem, key, value, conv_w, proj_w, e_w, e_b, token) for loc_attention_mem_step, or, without the location
-    weights, (mem, key, value, token) for dot_attention_mem_step."""
+    """-> (mem, key, value, conv_w, proj_w, e_w, e_b, token) for loc_attention_mem_step / loc_attention_heads_mem_step,
+    or, without the location weights, (mem, key, value, token) for dot_attention_mem_step."""
     mem = AttnMem()
     loc_w = tuple(w for w in (conv_w, proj_w, e_w, e_b) if w is not None)
     if len(loc_w) not in (0, 4):
@@ -1311,6 +1312,109 @@ def dot_attention_mem_step(mem, token, q, key, value, enc_len, num_head, tempera
     """-> (context [R,E], attn [R,T]) with R = B * num_head rows; mem, key, value and token come from
     attention_memory(key, value)."""
     return DotAttnMemStepFn.apply(mem, token, q, key, value, enc_len, num_head, temperature)
+
+
+# ----------------------------------------------------------------------------------------------------------
+ATTN_SMEM_OPTIN = 232448      # sm_90's opt-in shared memory per block (the library's value when no device is visible)
+
+
+def loc_attention_heads_supported(N, T, D, E, K, R):
+    """The limits of b200asr_locattn_heads_fwd / _bwd_acc (include/b200asr.h): N, K <= 16, D <= 512, E % 4 == 0,
+    E / CS <= 1024 and both kernels' shared memory within the device's opt-in maximum."""
+    if not (N > 0 and T > 0 and D > 0 and E > 0 and K > 0 and R >= 0):
+        return False
+    if N > 16 or K > 16 or D > 512 or E % 4 != 0:
+        return False
+    cs = 4
+    while cs > 1 and (E % (4 * cs) != 0 or (T < 8 * cs and E // (cs // 2) <= 1024)):
+        cs >>= 1
+    if E // cs > 1024:
+        return False
+    W, TP, TS, TT = 2 * R + 1, T + 2 * R, (T + cs - 1) // cs, 16
+    common = N * TP + K * N * W + D * K + D + N * D
+    fwd = 4 * ((common + N * T + K * TS + 3) // 4 * 4 + 512 * 4)
+    bwd = 4 * (common + D * K + N * D + 2 * N * T + N * cs * T + K * TT + 2 * TT * D + K * TP)
+    optin = ATTN_SMEM_OPTIN
+    if torch.cuda.is_available():
+        optin = torch.cuda.get_device_properties(torch.cuda.current_device()).shared_memory_per_block_optin
+    return max(fwd, bwd) + 32 * 4 <= optin      # + the kernels' static reduction scratch
+
+
+class LocAttnHeadsMemStepFn(Function):
+    """One multi-head location-aware attention step (src/module.py:215-258 with num_head = N > 1) on an attention
+    memory: forward = b200asr_locattn_heads_fwd (one launch: one location convolution per utterance shared by its N
+    heads); backward = b200asr_locattn_heads_bwd_acc (d(key) and the weight partials added into the memory, d(prev)
+    for all N channels, no d(value) write; AttnMemFn forms d(value) once after the loop over the B*N rows)."""
+
+    @staticmethod
+    def forward(ctx, mem, token, q, key, value, prev_att, enc_len, num_head, conv_w, proj_w, e_w, e_b, temperature):
+        ctx.set_materialize_grads(False)
+        lib = L.load()
+        q, prev_att = _f32c(q), _f32c(prev_att)
+        rows, T, D = key.shape
+        E = value.shape[2]
+        N = int(num_head)
+        B = rows // N
+        K, _, W = conv_w.shape
+        R = (W - 1) // 2
+        dev = key.device
+        enc_len = enc_len.to(device=dev, dtype=torch.int64).contiguous()
+        cw, pw = _f32c(conv_w.detach()), _f32c(proj_w.detach())
+        ew, eb = _f32c(e_w.detach()).view(-1), _f32c(e_b.detach()).view(-1)
+        attn = torch.empty((rows, T), device=dev, dtype=torch.float32)
+        cvec = torch.empty((rows, E), device=dev, dtype=torch.float32)
+        # algorithmic bytes: key + value read once; q, prev, attn, ctx, the weights, lengths
+        nbytes = 4 * rows * T * (D + E) + 4 * rows * (D + 2 * T + E) + 4 * (K * N * W + D * K + D + 1) + 8 * B
+        with L.timed("locattn_heads_fwd", nbytes):
+            L.check(lib.b200asr_locattn_heads_fwd(L.ptr(q), L.ptr(key), L.ptr(value), L.ptr(prev_att), L.ptr(enc_len),
+                                                  L.ptr(cw), L.ptr(pw), L.ptr(ew), L.ptr(eb), float(temperature), B, N,
+                                                  T, D, E, K, R, L.ptr(attn), L.ptr(cvec), L.stream()),
+                    "locattn_heads_fwd")
+        ctx.save_for_backward(q, key, value, prev_att, enc_len, cw, pw, ew, attn)
+        ctx.mem = mem
+        ctx.dims = (B, N, T, D, E, K, R)
+        ctx.temperature = float(temperature)
+        return cvec, attn
+
+    @staticmethod
+    def backward(ctx, dctx, dattn):
+        lib = L.load()
+        q, key, value, prev_att, enc_len, cw, pw, ew, attn = ctx.saved_tensors
+        B, N, T, D, E, K, R = ctx.dims
+        rows, W = B * N, 2 * R + 1
+        mem = ctx.mem
+        dev = key.device
+        CS = lib.b200asr_locattn_cluster_size(T, E)
+        P = lib.b200asr_locattn_heads_wpart_floats(N, D, K, R)
+        if mem.dkey is None:
+            mem.dkey = torch.zeros((rows, T, D), device=dev, dtype=torch.float32)
+            mem.wpart = torch.zeros((B * CS, P), device=dev, dtype=torch.float32)
+        dctx = _f32c(dctx) if dctx is not None else torch.zeros((rows, E), device=dev)
+        dattn = _f32c(dattn) if dattn is not None else None
+        dq_part = torch.empty((rows, CS, D), device=dev, dtype=torch.float32)
+        dprev = torch.empty((B, N, T), device=dev, dtype=torch.float32)
+        # value read once, key read and d(key) read + written once; q, prev, d(prev), attn, dattn, dctx, dq partials,
+        # the weights, the weight partials read + written, lengths
+        nbytes = (4 * rows * T * (3 * D + E) + 4 * rows * (D + 4 * T + E + CS * D) + 4 * (K * N * W + D * K + D)
+                  + 8 * B * CS * P + 8 * B)
+        with L.timed("locattn_heads_bwd_acc", nbytes):
+            L.check(lib.b200asr_locattn_heads_bwd_acc(L.ptr(q), L.ptr(key), L.ptr(value), L.ptr(prev_att),
+                                                      L.ptr(enc_len), L.ptr(cw), L.ptr(pw), L.ptr(ew), ctx.temperature,
+                                                      L.ptr(attn), L.ptr(dctx), L.ptr(dattn), B, N, T, D, E, K, R,
+                                                      L.ptr(dq_part), L.ptr(mem.dkey), L.ptr(dprev), L.ptr(mem.wpart),
+                                                      L.stream()), "locattn_heads_bwd_acc")
+        mem.attn.append(attn)
+        mem.dctx.append(dctx)
+        token_grad = torch.zeros(1, device=dev, dtype=torch.float32)
+        return (None, token_grad, dq_part.sum(1), None, None, dprev, None, None, None, None, None, None, None)
+
+
+def loc_attention_heads_mem_step(mem, token, q, key, value, prev_att, enc_len, num_head, conv_w, proj_w, e_w, e_b,
+                                 temperature):
+    """-> (context [R,E], attn [R,T]) with R = B * num_head rows, prev_att [B,N,T], conv_w [K,N,2R+1]; key ... e_b and
+    token come from attention_memory()."""
+    return LocAttnHeadsMemStepFn.apply(mem, token, q, key, value, prev_att, enc_len, num_head, conv_w, proj_w, e_w,
+                                       e_b, temperature)
 
 
 # ----------------------------------------------------------------------------------------------------------

@@ -230,6 +230,39 @@ B200ASR_API int b200asr_dotattn_bwd_acc(const float* q, const float* key, const 
                                         const float* dattn, int R, int T, int D, int E, float* dq_part, float* dkey_acc,
                                         b200asr_stream stream);
 
+/* ---- K12h: multi-head location-aware attention step, forward and decode-loop backward -----------------------------
+ * replaces src/module.py:234-258 (LocationAwareAttention.forward) + :189-195 (_attend) with num_head = N > 1.  ONE
+ * location convolution per utterance over the N channels of prev_att, its projection shared by the N heads:
+ *   conv[b,k,t] = sum_n sum_j w_conv[k,n,j] prev_att[b,n,t+j-R],  loc[b,t,d] = tanh(sum_k w_proj[d,k] conv[b,k,t]),
+ *   e[r,t] = (b_energy + sum_d w_energy[d] tanh(key[r,t,d] + q[r,d] + loc[r/N,t,d])) / temperature for t < len,
+ *   attn [R,T] = softmax(e) over t < len (exactly 0 at t >= len), ctx [R,E] = sum_t attn[t] value[r,t],
+ * with R = B * N rows (row r = b * N + n), len = clamp(enc_len[r / N], 0, T):
+ *   q [R,D], key [R,T,D], value [R,T,E] (the tensor Attention.forward forms, including its value.repeat(N, 1, 1)
+ *   without a value projection), prev_att [B,N,T], enc_len [B] i64, w_conv [K,N,2R+1], w_proj [D,K], w_energy [D],
+ *   b_energy [1].
+ * backward (the decode loop's form, as b200asr_locattn_bwd_acc): dctx [R,E], dattn [R,T] or NULL -> dq_part [R,CS,D]
+ *   (sum over CS = dq), dkey_acc [R,T,D] += d(key) for t < len, dprev [B,N,T], wpart_acc [B*CS, P] += the per-CTA
+ *   partials, P = b200asr_locattn_heads_wpart_floats(N, D, K, R) = D*K + K*N*(2R+1) + D + 1 laid out (d w_proj |
+ *   d w_conv | d w_energy | d b_energy).  No d(value): b200asr_attn_dvalue forms it once after the loop over R rows.
+ * One cluster of CS = b200asr_locattn_cluster_size(T, E) CTAs per UTTERANCE covers its N heads.  Frames t >= len of
+ * key and value are never read.  Deterministic: no float atomics.  An utterance with enc_len 0 gets the reference's
+ * NaN attention, context and d(value).  Limits (b200asr_locattn_heads_supported, checked before any CUDA call):
+ * N <= 16, K <= 16, D <= 512, E % 4 == 0, E / CS <= 1024, and both kernels' shared memory within the device's opt-in
+ * maximum (it grows as N (T + 2R) + K N (2R+1) + N CS T).                                                           */
+B200ASR_API int b200asr_locattn_heads_supported(int N, int T, int D, int E, int K, int R);
+B200ASR_API size_t b200asr_locattn_heads_wpart_floats(int N, int D, int K, int R);
+B200ASR_API int b200asr_locattn_heads_fwd(const float* q, const float* key, const float* value, const float* prev_att,
+                                          const long long* enc_len, const float* w_conv, const float* w_proj,
+                                          const float* w_energy, const float* b_energy, float temperature, int B,
+                                          int N, int T, int D, int E, int K, int R, float* attn, float* ctx,
+                                          b200asr_stream stream);
+B200ASR_API int b200asr_locattn_heads_bwd_acc(const float* q, const float* key, const float* value,
+                                              const float* prev_att, const long long* enc_len, const float* w_conv,
+                                              const float* w_proj, const float* w_energy, float temperature,
+                                              const float* attn, const float* dctx, const float* dattn, int B, int N,
+                                              int T, int D, int E, int K, int R, float* dq_part, float* dkey_acc,
+                                              float* dprev, float* wpart_acc, b200asr_stream stream);
+
 /* ---- K15: cross-entropy (log-softmax + NLL, ignore_index) forward + logit gradient ----------------------
  * replaces torch.nn.CrossEntropyLoss(ignore_index=0) at bin/train_asr.py:47,127-131.  row_loss [n_rows] =
  * lse(x) - x[target] (0 for ignored rows); dlogits (optional) = grad_scale[0] * (softmax(x) - onehot), zero rows

@@ -29,6 +29,9 @@ B200ASR_API int b200asr_debug_ctc_variant(int L_max);
 B200ASR_API int b200asr_debug_locattn_bwd_minb(int B, int T, int D, int E);
 /* test: the same for the dot-product attention backward b200asr_dotattn_bwd_acc launches for R rows. */
 B200ASR_API int b200asr_debug_dotattn_bwd_minb(int R, int T, int E);
+/* test: the same for the multi-head location-aware backward b200asr_locattn_heads_bwd_acc launches for B utterances
+ * of N heads (one cluster per utterance). */
+B200ASR_API int b200asr_debug_locattn_heads_bwd_minb(int B, int N, int T, int D, int E);
 /* test: the split-K plan b200asr_gemm3x_tn (form 0; 1 with B_lo), _nn (2), _nt (3) or b200asr_gemm_f16x3 (4) makes
  * for these sizes on the current device (132 SMs without one) with a workspace of workspace_bytes.  K is the
  * contraction length (T for nt, which walks `batches` entries of T; batches must be 1 for the other forms; the
