@@ -1550,9 +1550,19 @@ extern "C" int b200asr_debug_lstm_variant(int B, int H, int ndir, int bwd, int* 
     return 0;
 }
 
+extern "C" int b200asr_debug_lstm_cluster(int B, int H, int ndir, int bwd) {
+    Plan pl;
+    LstmVariant v;
+    if (B <= 0 || H <= 0 || (ndir != 1 && ndir != 2)) return -1;
+    const int rc = lstm_variant(B, H, ndir, bwd != 0, &pl, &v);
+    if (rc != 0) return rc;
+    return (bwd && v.gen == 1) ? lstm_umma_bwd_cluster(B, H, ndir) : 1;
+}
+
 extern "C" void b200asr_debug_set_lstm_mode(int mode) {
     g_lstm_mode = mode & 3;
     g_lstm_strict = (mode & 256) != 0;
+    lstm_umma_set_cluster_cap((mode >> 4) & 7);
 }
 
 extern "C" int b200asr_bilstm_fwd(float* gates, const float* w_hh, float* cstate, float* out, int B, int T, int H,

@@ -352,20 +352,52 @@ __device__ __forceinline__ float add_ftz(float a, float b) {
     asm("add.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
     return r;
 }
+// ---- distributed shared memory of a thread-block cluster ------------------------------------------------------------
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, int rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ void st_cluster_v2(uint32_t addr, uint32_t a, uint32_t b) {
+    asm volatile("st.relaxed.cluster.shared::cluster.v2.u32 [%0], {%1,%2};" ::"r"(addr), "r"(a), "r"(b) : "memory");
+}
+__device__ __forceinline__ uint2 ld_cluster_v2(uint32_t addr) {
+    uint2 v;
+    asm volatile("ld.relaxed.cluster.shared::cta.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 
 constexpr int ULB_EPI_WARPS = 16;
 constexpr int ULB_CTRL = 4;
+constexpr size_t ULB_SMEM_FIXED = 16384 + 128 + 128;   // A tiles, row scales, barriers (+ 2 H 128 B of W_hh)
+
+// Bytes of the cluster staging buffers: two parity buffers of the partials that the CS - 1 other ranks send to the
+// destinations this rank aggregates (nub / CS of them, 32 x UB fp32 each).
+__host__ __device__ inline size_t ulb_staging_bytes(int nub, int UB, int CS) {
+    return CS > 1 ? (size_t)2 * (CS - 1) * (nub / CS) * UL_BC * UB * 4 : 0;
+}
 
 // The state exchange is "data is the flag": every fp32 partial carries the parity of its buffer generation in its
 // least significant mantissa bit (2^-24 relative - below the resolution of the hi/lo product), the destination polls
 // its inbox IN GLOBAL MEMORY (L2) with relaxed loads until every word shows the expected tag and sums straight from
 // registers (flushing subnormals, so that a tagged zero adds nothing): no fence, no counter, no bulk copy, no
 // shared-memory inbox.
+// Two-level exchange (CS > 1): the CTAs of one (direction, batch group) run as clusters of CS consecutive unit blocks.
+// Cluster rank d % CS aggregates the cluster's partials for destination d: the other ranks store theirs into its
+// staging buffer in distributed shared memory (tagged the same way, two parity buffers), it polls its own shared
+// memory, sums the CS contributions in rank order with flushing adds, re-tags the sum and stores it to d's L2 inbox.
+// A destination then polls nub / CS sources (one per cluster) instead of nub, and the L2 traffic per step drops CS x.
 // Warp roles: warps [0, 16) pointwise + MMA + drain; lane 0 of warp 17 loads W_hh.  Warps 16 and 18 .. 20 have no work
 // but stay in the block: __launch_bounds__ and ul_launch_bwd's occupancy check count them.
-template <int UB>
+template <int UB, int CS>
 __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm_bwd_umma_kernel(UlParams p) {
     constexpr int KS = (4 * UB) / 16;               // MMAs (k-steps of 16) per product and n-block
+    // the 64 columns of a warpgroup's n-block start on a multiple of UB * CS units, so the aggregating rank of each
+    // accumulator column group depends only on its offset inside the block
+    static_assert(64 % (UB * CS) == 0, "cluster size");
     extern __shared__ __align__(1024) uint8_t smem[];
     const int H = p.H, T = p.T, nub = p.nub;
     const int NB = (H + 255) / 256;                 // n-blocks of (up to) 256 columns, 64 per warpgroup
@@ -377,14 +409,23 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
     uint64_t* a_ready = reinterpret_cast<uint64_t*>(rscale + 32);
     uint64_t* mma_done = a_ready + 1;               // the MMAs of a step have read the A tiles (one arrival per warp)
     uint64_t* wload = a_ready + 2;
+    // [parity][CS - 1 sender slots][nub / CS destinations][UL_BC][UB] fp32 (CS > 1)
+    float* stg = reinterpret_cast<float*>(sA1 + ULB_SMEM_FIXED);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     int blk = blockIdx.x;
     const int ub = blk % p.nub; blk /= p.nub;
     const int bg = blk % p.nbg; blk /= p.nbg;
     const int dir = blk;
+    const int crank = ub % CS;                      // = the block's rank in its cluster (clusters along unit blocks)
+    const int nsrc = nub / CS;                      // sources per L2 inbox: one per cluster
+    constexpr int PB = 32 / CS;                     // sources polled as one block (registers)
 
     for (int i = tid; i < 16384 / 16; i += blockDim.x) reinterpret_cast<uint4*>(sA1)[i] = make_uint4(0, 0, 0, 0);
+    if (CS > 1) {                                   // generation tags start at 0
+        for (int i = tid; i < (int)(ulb_staging_bytes(nub, UB, CS) / 16); i += blockDim.x)
+            reinterpret_cast<uint4*>(stg)[i] = make_uint4(0, 0, 0, 0);
+    }
     if (tid == 0) {
         mbar_init(a_ready, ULB_EPI_WARPS);
         mbar_init(mma_done, ULB_EPI_WARPS);
@@ -392,9 +433,11 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
         mbar_fence_init();
     }
     fence_proxy_async_smem();
-    __syncthreads();
-    const size_t xelems = (size_t)nub * nub * UL_BC * UB;                       // one parity buffer of one (dir, bg)
+    if (CS > 1) cluster_sync_all();                 // every peer runs and has zeroed its staging before a remote store
+    else __syncthreads();
+    const size_t xelems = (size_t)nub * nsrc * UL_BC * UB;                      // one parity buffer of one (dir, bg)
     float* xb = reinterpret_cast<float*>(p.xbuf) + ((size_t)dir * p.nbg + bg) * 2 * xelems;
+    const uint32_t stg_base = smem_u32(stg), stg_slot = (uint32_t)nsrc * (UL_BC * UB * 4);   // bytes per sender slot
 
     if (warp >= ULB_EPI_WARPS) {
         if (warp == ULB_EPI_WARPS + 1 && lane == 0) {
@@ -436,30 +479,30 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
             }
             if (step > 0) {
                 if (cell) {
-                    const float* ib = xb + (size_t)((step - 1) & 1) * xelems + (size_t)ub * nub * UL_BC * UB +
+                    const float* ib = xb + (size_t)((step - 1) & 1) * xelems + (size_t)ub * nsrc * UL_BC * UB +
                                       (size_t)b * UB + u;                       // [src] stride UL_BC * UB
                     const uint32_t tag = (uint32_t)(((step - 1) >> 1) & 1) ^ 1u;
                     const long long t0 = clock64();
                     float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-                    for (int sb = 0; sb < nub; sb += 32) {
-                        // cheap spin on one word, then the block of 32 sources (they finish within a few hundred cycles)
-                        float v[32];
-                        const int nhere = min(32, nub - sb);          // nub = 40 at H = 640: a tail block of 8 sources
+                    for (int sb = 0; sb < nsrc; sb += PB) {
+                        // cheap spin on one word, then the block of PB sources (they finish within a few hundred cycles)
+                        float v[PB];
+                        const int nhere = min(PB, nsrc - sb);         // nub = 40 at H = 640: a tail block of 8 sources
                         v[0] = ld_relaxed_f32(ib + (size_t)sb * UL_BC * UB);
                         while ((__float_as_uint(v[0]) & 1u) != tag) {
                             ul_watchdog(t0, p.err_flag);
                             v[0] = ld_relaxed_f32(ib + (size_t)sb * UL_BC * UB);
                         }
 #pragma unroll
-                        for (int j = 1; j < 32; ++j)
+                        for (int j = 1; j < PB; ++j)
                             v[j] = (j < nhere) ? ld_relaxed_f32(ib + (size_t)(sb + j) * UL_BC * UB) : __uint_as_float(tag);
                         uint32_t pending = 0;
 #pragma unroll
-                        for (int j = 1; j < 32; ++j) pending |= ((__float_as_uint(v[j]) & 1u) != tag) ? (1u << j) : 0u;
+                        for (int j = 1; j < PB; ++j) pending |= ((__float_as_uint(v[j]) & 1u) != tag) ? (1u << j) : 0u;
                         while (pending) {
                             ul_watchdog(t0, p.err_flag);
 #pragma unroll
-                            for (int j = 1; j < 32; ++j)
+                            for (int j = 1; j < PB; ++j)
                                 if (pending & (1u << j)) {
                                     v[j] = ld_relaxed_f32(ib + (size_t)(sb + j) * UL_BC * UB);
                                     if ((__float_as_uint(v[j]) & 1u) == tag) pending &= ~(1u << j);
@@ -468,8 +511,8 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
                         // flush-to-zero adds: a zero partial arrives with its tag as the smallest subnormal, and a
                         // zero dout row must still get dG = 0 exactly (same FADD instruction, no extra work)
 #pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            if (j < nhere) {                          // nub is a multiple of 4 (ulb_plan)
+                        for (int j = 0; j < PB; j += 4) {
+                            if (j < nhere) {                          // nub / CS is a multiple of 4 (ulb_plan)
                                 s0 = add_ftz(s0, v[j]); s1 = add_ftz(s1, v[j + 1]);
                                 s2 = add_ftz(s2, v[j + 2]); s3 = add_ftz(s3, v[j + 3]);
                             }
@@ -541,18 +584,70 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
                     const float* v1 = d + 16;
                     const float rs = rscale[drow];
                     const float k = 1.f / 2048.f;
+                    const uint32_t tagw = (uint32_t)((step >> 1) & 1) ^ 1u;
+                    // CS = 1: every partial to its destination's L2 inbox.  CS > 1: the partials another rank
+                    // aggregates go to that rank's staging buffer first; this rank's own share (column group
+                    // m = 4 hh + g with aggregator (8 m / UB) % CS == crank, the idx-th such group) waits in own[] for
+                    // the second pass, after these stores are on their way.
+                    constexpr int G = UB / 8;                  // column groups of 8 per destination
+                    float own[16 / CS];
 #pragma unroll
                     for (int hh = 0; hh < 2; ++hh) {
 #pragma unroll
                         for (int g = 0; g < 4; ++g) {
                             const float* v = hh ? &v1[4 * g] : &v0[4 * g];
-                            const int n = 256 * j + 64 * jq + 32 * hh + 8 * g + 2 * tq;
+                            const int m = 4 * hh + g;
+                            const int n = 256 * j + 64 * jq + 8 * m + 2 * tq;
                             const int dst = n / UB, uu = n - dst * UB;
+                            const int agg = (8 * m / UB) % CS;         // = dst % CS
                             const float o0 = (v[0] + v[2] * k) * rs;
                             const float o1 = (v[1] + v[3] * k) * rs;
-                            float* optr = outbase + (((size_t)dst * nub + ub) * UL_BC + drow) * UB + uu;
-                            const uint32_t tagw = (uint32_t)((step >> 1) & 1) ^ 1u;
-                            st_relaxed_v2(optr, (__float_as_uint(o0) & ~1u) | tagw, (__float_as_uint(o1) & ~1u) | tagw);
+                            if (CS > 1 && agg == crank) {
+                                const int idx = (m / G) / CS * G + m % G;
+                                own[2 * idx] = o0;
+                                own[2 * idx + 1] = o1;
+                                continue;
+                            }
+                            const uint32_t w0 = (__float_as_uint(o0) & ~1u) | tagw, w1 = (__float_as_uint(o1) & ~1u) | tagw;
+                            if (CS == 1) {
+                                st_relaxed_v2(outbase + (((size_t)dst * nsrc + ub) * UL_BC + drow) * UB + uu, w0, w1);
+                            } else {
+                                const int slot = (crank - agg - 1 + CS) % CS;
+                                const uint32_t sa = stg_base + (uint32_t)((step & 1) * (CS - 1) + slot) * stg_slot +
+                                                    (uint32_t)(((dst / CS) * UL_BC + drow) * UB + uu) * 4u;
+                                st_cluster_v2(mapa_shared(sa, agg), w0, w1);
+                            }
+                        }
+                    }
+                    if (CS > 1) {
+                        const long long t0 = clock64();
+#pragma unroll
+                        for (int idx = 0; idx < 8 / CS; ++idx) {
+                            const int m = G * (crank + CS * (idx / G)) + idx % G;
+                            const int n = 256 * j + 64 * jq + 8 * m + 2 * tq;
+                            const int dst = n / UB, uu = n - dst * UB;
+                            const uint32_t soff = (uint32_t)(((dst / CS) * UL_BC + drow) * UB + uu) * 4u;
+                            // the CS contributions in rank order; flushing adds drop the tagged zeros
+                            float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+                            for (int rr = 0; rr < CS; ++rr) {
+                                float x0 = own[2 * idx], x1 = own[2 * idx + 1];
+                                if (rr != crank) {
+                                    const int slot = (rr - crank - 1 + CS) % CS;
+                                    const uint32_t sa = stg_base + (uint32_t)((step & 1) * (CS - 1) + slot) * stg_slot + soff;
+                                    uint2 w = ld_cluster_v2(sa);
+                                    while (((w.x & 1u) != tagw) || ((w.y & 1u) != tagw)) {
+                                        ul_watchdog(t0, p.err_flag);
+                                        w = ld_cluster_v2(sa);
+                                    }
+                                    x0 = __uint_as_float(w.x);
+                                    x1 = __uint_as_float(w.y);
+                                }
+                                s0 = add_ftz(s0, x0);
+                                s1 = add_ftz(s1, x1);
+                            }
+                            st_relaxed_v2(outbase + (((size_t)dst * nsrc + ub / CS) * UL_BC + drow) * UB + uu,
+                                          (__float_as_uint(s0) & ~1u) | tagw, (__float_as_uint(s1) & ~1u) | tagw);
                         }
                     }
                 }
@@ -561,6 +656,7 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
             }
         }
     }
+    if (CS > 1) cluster_sync_all();                 // no peer accesses this block's shared memory after it exits
 }
 
 struct UlPlan {
@@ -628,10 +724,74 @@ int ul_launch_fwd(const UlPlan& pl, UlParams p, const float* w_hh, cudaStream_t 
 
 struct UlbPlan {
     int UB, nub, nbg, ctas, Bsub, nsplit;
+    int CS;                // cluster size of the two-level exchange (1: every partial straight to L2)
     size_t smem, pack_bytes, xbuf_bytes;
 };
 
-int ulb_plan(int B, int H, int ndir, UlbPlan* out) {
+int g_ulb_cs_cap = 0;              // test cap on CS (debug lstm mode bits 4..6; 0: none)
+bool g_ulb_coop_refused = false;   // the runtime refused a cooperative cluster launch: CS = 1 from then on
+
+const void* ulb_kernel(int UB, int CS) {
+    if (UB == 16)
+        return CS == 4 ? (const void*)bilstm_bwd_umma_kernel<16, 4>
+                       : CS == 2 ? (const void*)bilstm_bwd_umma_kernel<16, 2> : (const void*)bilstm_bwd_umma_kernel<16, 1>;
+    return CS == 4 ? (const void*)bilstm_bwd_umma_kernel<8, 4>
+                   : CS == 2 ? (const void*)bilstm_bwd_umma_kernel<8, 2> : (const void*)bilstm_bwd_umma_kernel<8, 1>;
+}
+
+void ulb_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, int ctas, int CS, size_t smem,
+                       cudaStream_t stream) {
+    *cfg = cudaLaunchConfig_t{};
+    cfg->gridDim = dim3(ctas);
+    cfg->blockDim = dim3(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL));
+    cfg->dynamicSmemBytes = smem;
+    cfg->stream = stream;
+    attr[0].id = cudaLaunchAttributeCooperative;    // every CTA of the launch co-resident, as the exchange needs
+    attr[0].val.cooperative = 1;
+    attr[1].id = cudaLaunchAttributeClusterDimension;
+    attr[1].val.clusterDim.x = CS;
+    attr[1].val.clusterDim.y = 1;
+    attr[1].val.clusterDim.z = 1;
+    cfg->attrs = attr;
+    cfg->numAttrs = 2;
+}
+
+// Clusters of CS blocks of this instance that the device holds at once (0 when it cannot be asked: no device, or a
+// runtime without the query).
+int ulb_max_clusters(int UB, int CS, int ctas, size_t smem) {
+    const void* fn = ulb_kernel(UB, CS);
+    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+        (void)cudaGetLastError();
+        return 0;
+    }
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr[2];
+    ulb_launch_config(&cfg, attr, ctas, CS, smem, 0);
+    cfg.attrs = attr + 1;                           // the occupancy query takes the cluster shape only
+    cfg.numAttrs = 1;
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, fn, &cfg) != cudaSuccess) {
+        (void)cudaGetLastError();
+        return 0;
+    }
+    return n;
+}
+
+// The largest CS in {4, 2} whose staging buffers fit in shared memory, that divides nub into a multiple of 4 sources
+// per inbox, and whose clusters the device holds all at once; else 1.
+int ulb_cluster(const UlbPlan& pl, size_t cap) {
+    for (int cs = 4; cs >= 2; cs >>= 1) {
+        if (g_ulb_coop_refused || (g_ulb_cs_cap != 0 && cs > g_ulb_cs_cap)) continue;
+        if (pl.nub % cs || (pl.nub / cs) % 4) continue;
+        const size_t smem = pl.smem + ulb_staging_bytes(pl.nub, pl.UB, cs);
+        if (smem > cap) continue;
+        if ((long long)ulb_max_clusters(pl.UB, cs, pl.ctas, smem) * cs < pl.ctas) continue;
+        return cs;
+    }
+    return 1;
+}
+
+int ulb_plan(int B, int H, int ndir, UlbPlan* out, bool cluster = true) {
     // accumulator = H columns in n-blocks of 256, 64 per warpgroup: 256 | 512 | 640 | 768 (a last block of 128 or 256)
     if (H % 128 != 0 || H < 256 || H > 768) return -1;
     const int sms = sm_count();
@@ -645,13 +805,15 @@ int ulb_plan(int B, int H, int ndir, UlbPlan* out) {
             const int ctas = ndir * nbg * nub;
             if (ctas > sms) continue;
             if (nub % 4) continue;
-            const size_t inbox = (size_t)nub * UL_BC * UB * 4;      // partials one destination receives per step
-            const size_t smem = (size_t)2 * H * 128 + 16384 + 128 + 128;
+            const size_t inbox = (size_t)nub * UL_BC * UB * 4;      // partials one destination receives per step (CS = 1)
+            const size_t smem = (size_t)2 * H * 128 + ULB_SMEM_FIXED;
             if (smem > cap || (inbox / ULB_CTRL) % 16 || (2 * H * 128) % 32768) continue;
             out->UB = UB; out->nub = nub; out->nbg = nbg; out->ctas = ctas; out->Bsub = Bs;
             out->nsplit = (B + Bs - 1) / Bs; out->smem = smem;
             out->pack_bytes = (size_t)ndir * nub * 2 * H * 128;
             out->xbuf_bytes = (size_t)ndir * nbg * 2 * nub * inbox;
+            out->CS = cluster ? ulb_cluster(*out, cap) : 1;
+            out->smem += ulb_staging_bytes(nub, UB, out->CS);
             return 0;
         }
         if (Bs <= UL_BC) break;
@@ -659,8 +821,10 @@ int ulb_plan(int B, int H, int ndir, UlbPlan* out) {
     return -2;
 }
 
+// One launch per row block.  A cooperative cluster launch that the runtime refuses runs nothing: the launches then
+// fall back to CS = 1 (and the planner never picks CS > 1 again in this process).
 template <int UB>
-int ul_launch_bwd(const UlbPlan& pl, UlParams p, const float* w_hh, cudaStream_t stream) {
+int ul_launch_bwd(UlbPlan pl, UlParams p, const float* w_hh, cudaStream_t stream) {
     {
         const long long n = (long long)p.ndir * pl.nub * 2 * p.H * 64;
         int blocks = (int)((n + 255) / 256);
@@ -668,34 +832,58 @@ int ul_launch_bwd(const UlbPlan& pl, UlParams p, const float* w_hh, cudaStream_t
         ul_pack_bwd_kernel<UB><<<blocks, 256, 0, stream>>>(w_hh, const_cast<uint8_t*>(p.wpack), p.H, p.ndir);
         B200_LAUNCH_CHECK("ul_pack_bwd_kernel");
     }
-    const void* fn = (const void*)bilstm_bwd_umma_kernel<UB>;
-    B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
-    int per_sm = 0;
-    const int threads = 32 * (ULB_EPI_WARPS + 1 + ULB_CTRL);
-    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, pl.smem));
-    B200_REQUIRE((long long)per_sm * sm_count() >= pl.ctas, "bilstm(umma bwd): %d CTAs cannot be co-resident (%d/SM x %d SMs)",
-                 pl.ctas, per_sm, sm_count());
-    for (int sp = 0; sp < pl.nsplit; ++sp) {
-        p.b0 = sp * pl.Bsub;
-        p.Bend = p.b0 + pl.Bsub < p.B ? p.b0 + pl.Bsub : p.B;
-        B200_CUDA(cudaMemsetAsync(p.counters, 0, UL_COUNTER_BYTES, stream));
-        B200_CUDA(cudaMemsetAsync(p.xbuf, 0, pl.xbuf_bytes, stream));     // generation tags start at 0
-        void* args[] = {&p};
-        B200_CUDA(cudaLaunchCooperativeKernel(fn, dim3(pl.ctas), dim3(threads), args, pl.smem, stream));
-        count_launch();
+    for (;;) {
+        const void* fn = ulb_kernel(UB, pl.CS);
+        B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
+        if (pl.CS == 1) {
+            int per_sm = 0;
+            B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 32 * (ULB_EPI_WARPS + 1 + ULB_CTRL),
+                                                                    pl.smem));
+            B200_REQUIRE((long long)per_sm * sm_count() >= pl.ctas,
+                         "bilstm(umma bwd): %d CTAs cannot be co-resident (%d/SM x %d SMs)", pl.ctas, per_sm, sm_count());
+        }
+        cudaLaunchConfig_t cfg;
+        cudaLaunchAttribute attr[2];
+        ulb_launch_config(&cfg, attr, pl.ctas, pl.CS, pl.smem, stream);
+        bool refused = false;
+        for (int sp = 0; sp < pl.nsplit; ++sp) {
+            p.b0 = sp * pl.Bsub;
+            p.Bend = p.b0 + pl.Bsub < p.B ? p.b0 + pl.Bsub : p.B;
+            B200_CUDA(cudaMemsetAsync(p.counters, 0, UL_COUNTER_BYTES, stream));
+            B200_CUDA(cudaMemsetAsync(p.xbuf, 0, pl.xbuf_bytes, stream));     // generation tags start at 0
+            void* args[] = {&p};
+            const cudaError_t e = cudaLaunchKernelExC(&cfg, fn, args);
+            if (e != cudaSuccess && pl.CS > 1 && sp == 0) {
+                (void)cudaGetLastError();
+                refused = true;
+                break;
+            }
+            B200_CUDA(e);
+            count_launch();
+        }
+        if (!refused) return B200_OK;
+        g_ulb_coop_refused = true;
+        pl.smem -= ulb_staging_bytes(pl.nub, UB, pl.CS);
+        pl.CS = 1;
     }
-    return B200_OK;
 }
 
 }  // namespace
 
 bool lstm_umma_bwd_variant(int B, int H, int ndir, int* ub, int* nsplit) {
     UlbPlan pl;
-    if (ulb_plan(B, H, ndir, &pl) != 0) return false;
+    if (ulb_plan(B, H, ndir, &pl, false) != 0) return false;
     *ub = pl.UB;
     *nsplit = pl.nsplit;
     return true;
 }
+
+int lstm_umma_bwd_cluster(int B, int H, int ndir) {
+    UlbPlan pl;
+    return ulb_plan(B, H, ndir, &pl) == 0 ? pl.CS : -1;
+}
+
+void lstm_umma_set_cluster_cap(int cap) { g_ulb_cs_cap = cap; }
 
 bool lstm_umma_fwd_variant(int B, int H, int ndir, int* ub, int* ubp, int* nsplit) {
     UlPlan pl;
@@ -730,7 +918,7 @@ size_t lstm_umma_workspace_bytes(int B, int H, int ndir) {
     UlbPlan pb;
     size_t f = 0, b = 0;
     if (ul_plan(B, H, ndir, &pl) == 0) f = ul_align(pl.pack_bytes) + ul_align(pl.xbuf_bytes) + UL_COUNTER_BYTES;
-    if (ulb_plan(B, H, ndir, &pb) == 0) b = ul_align(pb.pack_bytes) + ul_align(pb.xbuf_bytes) + UL_COUNTER_BYTES;
+    if (ulb_plan(B, H, ndir, &pb, false) == 0) b = ul_align(pb.pack_bytes) + ul_align(pb.xbuf_bytes) + UL_COUNTER_BYTES;
     return f > b ? f : b;
 }
 

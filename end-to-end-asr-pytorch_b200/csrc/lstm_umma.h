@@ -9,6 +9,10 @@ namespace b200asr {
 // launches.  false: no plan.
 bool lstm_umma_fwd_variant(int B, int H, int ndir, int* ub, int* ubp, int* nsplit);
 bool lstm_umma_bwd_variant(int B, int H, int ndir, int* ub, int* nsplit);
+// Cluster size of the backward's two-level exchange for these sizes on the current device (1: no clusters); < 0: no
+// plan.  cap > 0 limits it (debug lstm mode bits 4..6).
+int lstm_umma_bwd_cluster(int B, int H, int ndir);
+void lstm_umma_set_cluster_cap(int cap);
 int lstm_umma_bwd(float* gates, const float* w_hh, const float* cstate, const float* dout, int B, int T, int H, int ndir,
                   void* workspace, size_t workspace_bytes, cudaStream_t stream);
 size_t lstm_umma_workspace_bytes(int B, int H, int ndir);

@@ -49,6 +49,7 @@ SIGNATURES = {
     "b200asr_bilstm_bwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_debug_set_lstm_mode": (None, [c_int]),
     "b200asr_debug_lstm_variant": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_int)]),
+    "b200asr_debug_lstm_cluster": (c_int, [c_int, c_int, c_int, c_int]),
     "b200asr_debug_ctc_variant": (c_int, [c_int]),
     "b200asr_debug_locattn_bwd_minb": (c_int, [c_int, c_int, c_int, c_int]),
     "b200asr_debug_dotattn_bwd_minb": (c_int, [c_int, c_int, c_int]),

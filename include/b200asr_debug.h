@@ -10,8 +10,15 @@ extern "C" {
 /* debug/test: 0 (default) = wgmma step GEMMs where the shape allows, else 3xTF32 mma.sync wherever the planner finds
  * a 16-row-tile decomposition, else fp32 FMA; 1 = always the packed-fp32-FMA step kernels; 3 = never wgmma (the
  * mma.sync generation); 256 = as 0, with the formal acquire (ld.acquire + proxy fence) after each flag poll of the
- * wgmma forward.  All are fp32-class and parity-tested. */
+ * wgmma forward.  All are fp32-class and parity-tested.  Bits 4..6 ((mode >> 4) & 7, 0 = none) cap the cluster size
+ * of the wgmma backward's two-level exchange: 16 keeps it at 1 (every partial straight to L2), 32 at <= 2. */
 B200ASR_API void b200asr_debug_set_lstm_mode(int mode);
+/* test: the cluster size CS of the exchange b200asr_bilstm_bwd (bwd = 1) runs for these sizes under the current lstm
+ * mode on the current device: the largest of 4, 2 whose staging buffers fit in shared memory, that divides the unit
+ * blocks into a multiple of 4 clusters, and whose clusters the device holds all at once for a cooperative launch; else 1
+ * (also without a device, without the cluster occupancy query, after the runtime refused a cooperative cluster launch,
+ * and for every kernel but the wgmma backward).  < 0 when the shape has no plan. */
+B200ASR_API int b200asr_debug_lstm_cluster(int B, int H, int ndir, int bwd);
 /* test: the step-kernel variant b200asr_bilstm_fwd (bwd = 0) / _bwd (bwd = 1) runs for these sizes under the current
  * lstm mode on the current device (132 SMs / 232448 B of shared memory without one).  Fills desc[9] =
  * {generation (1 wgmma, 2 mma.sync 3xTF32, 3 fp32 FMA), unit block UB, template unit block (UBP of the wgmma forward,
