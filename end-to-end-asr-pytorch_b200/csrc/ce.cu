@@ -32,7 +32,8 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_kernel(const float* __restrict
         }
     }
     const float M = warp_max(m);
-    const float S = warp_sum((m == NEG_INF) ? 0.f : s * expf(m - M));
+    // a lane whose only finite-or-NaN values were NaN keeps m = -inf and s = NaN: s * 0 carries that NaN into S
+    const float S = warp_sum(s * ((m == NEG_INF) ? 0.f : expf(m - M)));
     const float lse = M + logf(S);
     if (lane == 0) row_loss[row] = lse - xr[t];
     if (dx) {

@@ -11,6 +11,7 @@
 namespace b200asr {
 
 __device__ __forceinline__ float np_logaddexp(float a, float b) {
+    if (a == b) return a + 0.6931471805599453f;             // numpy's branch: logaddexp(-inf, -inf) = -inf, not NaN
     const float m = fmaxf(a, b);
     const float d = -fabsf(a - b);
     return m + log1pf(expf(d));

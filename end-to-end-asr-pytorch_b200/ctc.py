@@ -28,13 +28,20 @@ class CTCPrefixScore:
 
     def cheap_compute_batch(self, prefixes, r_prevs, candidates):
         """prefixes: list of N token lists; r_prevs: [N, T, 2] device tensor (or list of [T,2]); candidates: [N, C]
-        int tensor / nested list.  Returns (psi [N, C], r [N, C, T, 2]) device tensors."""
+        host int tensor / nested list.  Returns (psi [N, C], r [N, C, T, 2]) device tensors.  Token ids outside
+        [0, V) raise ValueError before the launch (the kernel gathers log-probs at the candidate ids)."""
         lib = L.load()
         dev = self.x.device
+        V = self.odim
+        cand = torch.as_tensor(candidates, dtype=torch.int32).cpu()
+        if cand.numel() and (int(cand.min()) < 0 or int(cand.max()) >= V):
+            raise ValueError("CTCPrefixScore: candidate ids must lie in [0, %d)" % V)
+        if any(not 0 <= int(tok) < V for g in prefixes for tok in g):
+            raise ValueError("CTCPrefixScore: prefix tokens must lie in [0, %d)" % V)
         if not torch.is_tensor(r_prevs):
             r_prevs = torch.stack([torch.as_tensor(r, dtype=torch.float32).to(dev) for r in r_prevs])
         r_prevs = r_prevs.to(device=dev, dtype=torch.float32).contiguous()
-        cand = torch.as_tensor(candidates, dtype=torch.int32).to(dev).contiguous()
+        cand = cand.to(dev).contiguous()
         N, C = cand.shape
         T = self.input_length
         assert r_prevs.shape == (N, T, 2)
