@@ -32,8 +32,11 @@
 //
 // Reference behaviour restated: torch.nn.LSTM as called from /root/reference/src/module.py:112-113,129-132 (single
 // layer, batch_first, zero initial state, run over the zero-padded frames - no packing, SURVEY.md F5), gates i,f,g,o.
+// Every step kernel takes the pointwise cell as a template parameter (csrc/rnn_cell.cuh): the bigru_* kernels restate
+// torch.nn.GRU of an encoder layer (the same call site) on the packed 4-slot gate layout, with the same plan.
 #include "common.cuh"
 #include "lstm_umma.h"
+#include "rnn_cell.cuh"
 #include "../../include/b200asr.h"
 #include "../../include/b200asr_debug.h"
 
@@ -163,7 +166,7 @@ __device__ __forceinline__ float pick_row(const float (&acc)[R][4], int kq, int 
 
 // ------------------------------------------------------------------------------------------
 // Forward compute group: 128 threads = 32 register tiles (4 gates x R rows) x 4 K-chunks.  lane = kq*8 + tile%8.
-template <int R>
+template <int CELL, int R>
 __device__ __forceinline__ void fwd_group(const LstmParams& p, int g, int gt, int dir, int bg, int ub, const float4* Ws,
                                           const float* hsg, uint64_t* full, uint64_t* done, float* xbg,
                                           uint64_t* turn) {
@@ -287,15 +290,9 @@ __device__ __forceinline__ void fwd_group(const LstmParams& p, int g, int gt, in
             hq[i] = 0.f;
             const int b = bglob0 + i;
             if (has_tile && b < p.Bend) {
-                const float ig = sigmoidf_(gx[i].x + pick_row<R>(acc, kq, i, 0));
-                const float fg = sigmoidf_(gx[i].y + pick_row<R>(acc, kq, i, 1));
-                const float gg = tanhf(gx[i].z + pick_row<R>(acc, kq, i, 2));
-                const float og = sigmoidf_(gx[i].w + pick_row<R>(acc, kq, i, 3));
-                const float c = fmaf(fg, c_reg[i], ig * gg);
-                c_reg[i] = c;
-                hq[i] = og * tanhf(c);
-                cq[i] = c;
-                gq[i] = make_float4(ig, fg, gg, og);
+                cell_fwd<CELL>([&](int q) { return f4_at(gx[i], q) + pick_row<R>(acc, kq, i, q); }, c_reg[i], gq[i]);
+                hq[i] = cell_h<CELL>(gq[i], c_reg[i]);
+                cq[i] = c_reg[i];
             }
         }
         // publish the new state FIRST (it is on the critical path of every peer CTA), then write the stash
@@ -321,7 +318,9 @@ __device__ __forceinline__ void fwd_group(const LstmParams& p, int g, int gt, in
     }
 }
 
-__global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_fwd_kernel(LstmParams p) {
+// the kernel bodies take the cell (csrc/rnn_cell.cuh) as a template parameter; one __global__ per cell below each
+template <int CELL>
+__device__ __forceinline__ void fwd_kernel_body(const LstmParams& p) {
     extern __shared__ __align__(128) unsigned char s_raw[];
     const int H = p.H, UB = p.UB, Bc = p.Bc, T = p.T, NH = p.NH;
     const int Bh = Bc / NH;
@@ -377,16 +376,22 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_fwd_kernel(LstmParams 
     if (g >= NH) return;
     const int gt = tid - g * LSTM_GTHREADS;
     if (p.R == 8)
-        fwd_group<8>(p, g, gt, dir, bg, ub, Ws, hs + (size_t)g * hs_half, &full[g * LSTM_NCHUNK], &done[g],
+        fwd_group<CELL, 8>(p, g, gt, dir, bg, ub, Ws, hs + (size_t)g * hs_half, &full[g * LSTM_NCHUNK], &done[g],
                      xb + (size_t)g * 2 * half_elems, turn);
     else
-        fwd_group<4>(p, g, gt, dir, bg, ub, Ws, hs + (size_t)g * hs_half, &full[g * LSTM_NCHUNK], &done[g],
+        fwd_group<CELL, 4>(p, g, gt, dir, bg, ub, Ws, hs + (size_t)g * hs_half, &full[g * LSTM_NCHUNK], &done[g],
                      xb + (size_t)g * 2 * half_elems, turn);
+}
+__global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_fwd_kernel(LstmParams p) {
+    fwd_kernel_body<CELL_LSTM>(p);
+}
+__global__ void __launch_bounds__(LSTM_THREADS, 1) bigru_fwd_kernel(LstmParams p) {
+    fwd_kernel_body<CELL_GRU>(p);
 }
 
 // ------------------------------------------------------------------------------------------
 // Backward compute group.
-template <int R>
+template <int CELL, int R>
 __device__ __forceinline__ void bwd_group(const LstmParams& p, int g, int gt, int dir, int bg, int ub, const float* Wr,
                                           const float* inb, float* dgs, uint64_t* full, uint64_t* done, float* xbg,
                                           uint64_t* turn) {
@@ -468,14 +473,7 @@ __device__ __forceinline__ void bwd_group(const LstmParams& p, int g, int gt, in
             const int b = bglob0 + i;
             float4 dg = make_float4(0.f, 0.f, 0.f, 0.f);
             if (has_tile && b < p.Bend) {
-                const float ig = gtv[i].x, fg = gtv[i].y, gg = gtv[i].z, og = gtv[i].w;
-                const float tc = tanhf(ct[i]);
-                const float dc = dc_reg[i] + dh[i] * og * (1.f - tc * tc);
-                dg.x = dc * gg * ig * (1.f - ig);
-                dg.y = dc * cp[i] * fg * (1.f - fg);
-                dg.z = dc * ig * (1.f - gg * gg);
-                dg.w = dh[i] * tc * og * (1.f - og);
-                dc_reg[i] = dc * fg;
+                cell_bwd<CELL>(gtv[i], ct[i], cp[i], dh[i], dc_reg[i], dg);
                 const size_t row = ((size_t)dir * p.B + b) * T + tt;
                 *reinterpret_cast<float4*>(p.gates + (row * H + ug) * 4) = dg;
             }
@@ -582,7 +580,8 @@ __device__ __forceinline__ void bwd_group(const LstmParams& p, int g, int gt, in
 }
 
 // Shared memory: Wr[4UB][H] | inbox[NH][nub*Bh*UB] | dGs[NH][4UB*Bh] | barriers
-__global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_bwd_kernel(LstmParams p) {
+template <int CELL>
+__device__ __forceinline__ void bwd_kernel_body(const LstmParams& p) {
     extern __shared__ __align__(128) unsigned char s_raw[];
     const int H = p.H, UB = p.UB, Bc = p.Bc, T = p.T, nub = p.nub, NH = p.NH;
     const int Bh = Bc / NH;
@@ -639,11 +638,17 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_bwd_kernel(LstmParams 
     if (g >= NH) return;
     const int gt = tid - g * LSTM_GTHREADS;
     if (p.R == 8)
-        bwd_group<8>(p, g, gt, dir, bg, ub, Wr, inbox + (size_t)g * inbox_elems, dGs + (size_t)g * 4 * UB * Bh,
+        bwd_group<CELL, 8>(p, g, gt, dir, bg, ub, Wr, inbox + (size_t)g * inbox_elems, dGs + (size_t)g * 4 * UB * Bh,
                      &full[g * LSTM_NCHUNK], &done[g], xb + (size_t)g * 2 * nub * inbox_elems, turn);
     else
-        bwd_group<4>(p, g, gt, dir, bg, ub, Wr, inbox + (size_t)g * inbox_elems, dGs + (size_t)g * 4 * UB * Bh,
+        bwd_group<CELL, 4>(p, g, gt, dir, bg, ub, Wr, inbox + (size_t)g * inbox_elems, dGs + (size_t)g * 4 * UB * Bh,
                      &full[g * LSTM_NCHUNK], &done[g], xb + (size_t)g * 2 * nub * inbox_elems, turn);
+}
+__global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_bwd_kernel(LstmParams p) {
+    bwd_kernel_body<CELL_LSTM>(p);
+}
+__global__ void __launch_bounds__(LSTM_THREADS, 1) bigru_bwd_kernel(LstmParams p) {
+    bwd_kernel_body<CELL_GRU>(p);
 }
 
 
@@ -726,7 +731,7 @@ __global__ void lstm_pack_mma_kernel(const float* __restrict__ w, float* __restr
 // NS = number of k-step parities accumulated separately: a warp carries 6*NS independent MMA accumulator chains
 // (2 tiles x 3 products x NS); the dependent-issue latency of mma.sync is long enough that 6 chains leave the
 // tensor pipe idle.
-template <int NS>
+template <int CELL, int NS>
 __device__ __forceinline__ void fwd_group_mma(const LstmParams& p, int g, int gt, int dir, int bg, int ub,
                                               const float4* Wm, const float* hsg, uint64_t* full, uint64_t* done,
                                               float* xbg, uint64_t* turn) {
@@ -818,15 +823,11 @@ __device__ __forceinline__ void fwd_group_mma(const LstmParams& p, int g, int gt
         for (int i = 0; i < 2; ++i) {
             gq[i] = make_float4(0.f, 0.f, 0.f, 0.f);
             if (has_unit && brow[i] < p.Bend) {
-                const float ig = sigmoidf_(gx[i].x + t0[2 * i]);
-                const float fg = sigmoidf_(gx[i].y + t0[2 * i + 1]);
-                const float gg = tanhf(gx[i].z + t1[2 * i]);
-                const float og = sigmoidf_(gx[i].w + t1[2 * i + 1]);
-                const float c = fmaf(fg, c_reg[i], ig * gg);
-                c_reg[i] = c;
-                hq[i] = og * tanhf(c);
-                cq[i] = c;
-                gq[i] = make_float4(ig, fg, gg, og);
+                // slots (0, 1) come from tile t0, (2, 3) from t1
+                cell_fwd<CELL>([&](int q) { return f4_at(gx[i], q) + (q < 2 ? t0 : t1)[2 * i + (q & 1)]; }, c_reg[i],
+                               gq[i]);
+                hq[i] = cell_h<CELL>(gq[i], c_reg[i]);
+                cq[i] = c_reg[i];
             }
         }
         if (step + 1 < T) {
@@ -852,6 +853,7 @@ __device__ __forceinline__ void fwd_group_mma(const LstmParams& p, int g, int gt
 // scheduler has during the other group's turn; (b) the flat K loop is software-pipelined by hand over blocks of
 // four k-steps (two register stages), so that every shared-memory load is issued a whole block (24 MMAs) before
 // its first use.  Needs H % 128 == 0 (blocks of four k-steps never straddle a bulk-copy chunk).
+template <int CELL>
 __device__ __forceinline__ void fwd_group_mma_v2(const LstmParams& p, int g, int gt, int dir, int bg, int ub,
                                                  const float4* Wm, const float* hsg, uint64_t* full, uint64_t* done,
                                                  float* xbg, uint64_t* turn) {
@@ -948,15 +950,11 @@ __device__ __forceinline__ void fwd_group_mma_v2(const LstmParams& p, int g, int
         for (int i = 0; i < 2; ++i) {
             gq[i] = make_float4(0.f, 0.f, 0.f, 0.f);
             if (has_unit && brow[i] < p.Bend) {
-                const float ig = sigmoidf_(gx[i].x + t0[2 * i]);
-                const float fg = sigmoidf_(gx[i].y + t0[2 * i + 1]);
-                const float gg = tanhf(gx[i].z + t1[2 * i]);
-                const float og = sigmoidf_(gx[i].w + t1[2 * i + 1]);
-                const float c = fmaf(fg, c_reg[i], ig * gg);
-                c_reg[i] = c;
-                hq[i] = og * tanhf(c);
-                cq[i] = c;
-                gq[i] = make_float4(ig, fg, gg, og);
+                // slots (0, 1) come from tile t0, (2, 3) from t1
+                cell_fwd<CELL>([&](int q) { return f4_at(gx[i], q) + (q < 2 ? t0 : t1)[2 * i + (q & 1)]; }, c_reg[i],
+                               gq[i]);
+                hq[i] = cell_h<CELL>(gq[i], c_reg[i]);
+                cq[i] = c_reg[i];
             }
         }
         if (step + 1 < T) {
@@ -977,7 +975,8 @@ __device__ __forceinline__ void fwd_group_mma_v2(const LstmParams& p, int g, int
     }
 }
 
-__global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_fwd_mma_kernel(LstmParams p) {
+template <int CELL>
+__device__ __forceinline__ void fwd_mma_kernel_body(const LstmParams& p) {
     extern __shared__ __align__(128) unsigned char s_raw[];
     const int H = p.H, UB = p.UB, T = p.T, NH = p.NH;
     const int KC = H / LSTM_NCHUNK;
@@ -1029,17 +1028,24 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_fwd_mma_kernel(LstmPar
     const int g = tid / LSTM_GTHREADS;
     if (g >= NH) return;
     if (p.form == 0)
-        fwd_group_mma_v2(p, g, tid - g * LSTM_GTHREADS, dir, bg, ub, Wm, hs + (size_t)g * hs_half,
+        fwd_group_mma_v2<CELL>(p, g, tid - g * LSTM_GTHREADS, dir, bg, ub, Wm, hs + (size_t)g * hs_half,
                          &full[g * LSTM_NCHUNK], &done[g], xb + (size_t)g * 2 * half_elems, turn);
     else if (p.form == 2)
-        fwd_group_mma<2>(p, g, tid - g * LSTM_GTHREADS, dir, bg, ub, Wm, hs + (size_t)g * hs_half,
+        fwd_group_mma<CELL, 2>(p, g, tid - g * LSTM_GTHREADS, dir, bg, ub, Wm, hs + (size_t)g * hs_half,
                          &full[g * LSTM_NCHUNK], &done[g], xb + (size_t)g * 2 * half_elems, turn);
     else
-        fwd_group_mma<1>(p, g, tid - g * LSTM_GTHREADS, dir, bg, ub, Wm, hs + (size_t)g * hs_half,
+        fwd_group_mma<CELL, 1>(p, g, tid - g * LSTM_GTHREADS, dir, bg, ub, Wm, hs + (size_t)g * hs_half,
                          &full[g * LSTM_NCHUNK], &done[g], xb + (size_t)g * 2 * half_elems, turn);
+}
+__global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_fwd_mma_kernel(LstmParams p) {
+    fwd_mma_kernel_body<CELL_LSTM>(p);
+}
+__global__ void __launch_bounds__(LSTM_THREADS, 1) bigru_fwd_mma_kernel(LstmParams p) {
+    fwd_mma_kernel_body<CELL_GRU>(p);
 }
 
 // ---- backward group, tensor cores
+template <int CELL>
 __device__ __forceinline__ void bwd_group_mma(const LstmParams& p, int g, int gt, int dir, int bg, int ub,
                                               const float4* Wm, const float* inb, float* dgs, uint64_t* full,
                                               uint64_t* done, float* xbg, uint64_t* turn) {
@@ -1109,14 +1115,7 @@ __device__ __forceinline__ void bwd_group_mma(const LstmParams& p, int g, int gt
         for (int j = 0; j < 2; ++j) {
             float4 dg = make_float4(0.f, 0.f, 0.f, 0.f);
             if (it_ok[j]) {
-                const float ig = gtv[j].x, fg = gtv[j].y, gg = gtv[j].z, og = gtv[j].w;
-                const float tc = tanhf(ct[j]);
-                const float dc = dc_reg[j] + dh[j] * og * (1.f - tc * tc);
-                dg.x = dc * gg * ig * (1.f - ig);
-                dg.y = dc * cp[j] * fg * (1.f - fg);
-                dg.z = dc * ig * (1.f - gg * gg);
-                dg.w = dh[j] * tc * og * (1.f - og);
-                dc_reg[j] = dc * fg;
+                cell_bwd<CELL>(gtv[j], ct[j], cp[j], dh[j], dc_reg[j], dg);
                 const size_t row = ((size_t)dir * p.B + it_row[j]) * T + tt;
                 *reinterpret_cast<float4*>(p.gates + (row * H + ub * UB + it_u[j]) * 4) = dg;
             }
@@ -1189,7 +1188,8 @@ __device__ __forceinline__ void bwd_group_mma(const LstmParams& p, int g, int gt
     }
 }
 
-__global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_bwd_mma_kernel(LstmParams p) {
+template <int CELL>
+__device__ __forceinline__ void bwd_mma_kernel_body(const LstmParams& p) {
     extern __shared__ __align__(128) unsigned char s_raw[];
     const int H = p.H, UB = p.UB, Bc = p.Bc, T = p.T, nub = p.nub, NH = p.NH;
     float* Wr = reinterpret_cast<float*>(s_raw);
@@ -1239,9 +1239,15 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_bwd_mma_kernel(LstmPar
     }
     const int g = tid / LSTM_GTHREADS;
     if (g >= NH) return;
-    bwd_group_mma(p, g, tid - g * LSTM_GTHREADS, dir, bg, ub, reinterpret_cast<const float4*>(Wr),
+    bwd_group_mma<CELL>(p, g, tid - g * LSTM_GTHREADS, dir, bg, ub, reinterpret_cast<const float4*>(Wr),
                   inbox + (size_t)g * inbox_elems, dGs + (size_t)g * 4 * UB * 16, &full[g * LSTM_NCHUNK], &done[g],
                   xb + (size_t)g * 2 * nub * inbox_elems, turn);
+}
+__global__ void __launch_bounds__(LSTM_THREADS, 1) bilstm_bwd_mma_kernel(LstmParams p) {
+    bwd_mma_kernel_body<CELL_LSTM>(p);
+}
+__global__ void __launch_bounds__(LSTM_THREADS, 1) bigru_bwd_mma_kernel(LstmParams p) {
+    bwd_mma_kernel_body<CELL_GRU>(p);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1484,7 +1490,8 @@ extern "C" int b200asr_bilstm_uses_tensor_cores(int B, int H, int ndir) {
     return pl.mma ? 1 : 0;
 }
 
-static int bilstm_run(bool bwd, float* gates, const float* w_hh, float* cstate, float* out_or_dout, int B, int T,
+// cell: CELL_LSTM or CELL_GRU (csrc/rnn_cell.cuh).  Both cells take the same plan and variant.
+static int bilstm_run(int cell, bool bwd, float* gates, const float* w_hh, float* cstate, float* out_or_dout, int B, int T,
                       int H, int ndir, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     B200_REQUIRE(gates && w_hh && cstate && out_or_dout && workspace, "bilstm: null pointer");
     B200_REQUIRE(B > 0 && T > 0 && H > 0 && (ndir == 1 || ndir == 2), "bilstm: bad sizes B=%d T=%d H=%d ndir=%d", B, T,
@@ -1495,10 +1502,10 @@ static int bilstm_run(bool bwd, float* gates, const float* w_hh, float* cstate, 
                  "bilstm: no feasible decomposition for B=%d H=%d ndir=%d (H must be a multiple of 16)", B, H, ndir);
     B200_REQUIRE(workspace_bytes >= b200asr_bilstm_workspace_bytes(B, T, H, ndir), "bilstm: workspace too small");
     if (v.gen == 1 && !bwd)
-        return lstm_umma_fwd(gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes, v.strict != 0,
-                             stream);
+        return lstm_umma_fwd(cell, gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes,
+                             v.strict != 0, stream);
     if (v.gen == 1)
-        return lstm_umma_bwd(gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes, stream);
+        return lstm_umma_bwd(cell, gates, w_hh, cstate, out_or_dout, B, T, H, ndir, workspace, workspace_bytes, stream);
     unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
     float* packed = reinterpret_cast<float*>(ws);
     const size_t xoff = align_up(pl.pack_bytes, 256);
@@ -1519,8 +1526,13 @@ static int bilstm_run(bool bwd, float* gates, const float* w_hh, float* cstate, 
     p.gates = gates; p.whh = packed; p.cst = cstate; p.out = out_or_dout; p.xbuf = xbuf; p.counters = counters;
     p.err_flag = err_flag; p.B = B; p.T = T; p.H = H; p.ndir = ndir; p.UB = pl.UB; p.Bc = pl.Bc; p.nub = pl.nub;
     p.nbg = pl.nbg; p.NH = pl.NH; p.R = pl.R; p.mma = pl.mma; p.form = v.form;
-    const void* fn = !pl.mma ? (bwd ? (const void*)bilstm_bwd_kernel : (const void*)bilstm_fwd_kernel)
-                             : (bwd ? (const void*)bilstm_bwd_mma_kernel : (const void*)bilstm_fwd_mma_kernel);
+    const void* fn;
+    if (cell == CELL_GRU)
+        fn = !pl.mma ? (bwd ? (const void*)bigru_bwd_kernel : (const void*)bigru_fwd_kernel)
+                     : (bwd ? (const void*)bigru_bwd_mma_kernel : (const void*)bigru_fwd_mma_kernel);
+    else
+        fn = !pl.mma ? (bwd ? (const void*)bilstm_bwd_kernel : (const void*)bilstm_fwd_kernel)
+                     : (bwd ? (const void*)bilstm_bwd_mma_kernel : (const void*)bilstm_fwd_mma_kernel);
     const size_t smem = bwd ? pl.smem_bwd : pl.smem_fwd;
     B200_REQUIRE(smem <= (size_t)max_optin_smem(), "bilstm: %zu B of shared memory exceed the device limit", smem);
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1567,14 +1579,27 @@ extern "C" void b200asr_debug_set_lstm_mode(int mode) {
 
 extern "C" int b200asr_bilstm_fwd(float* gates, const float* w_hh, float* cstate, float* out, int B, int T, int H,
                                   int ndir, void* workspace, size_t workspace_bytes, b200asr_stream stream) {
-    return bilstm_run(false, gates, w_hh, cstate, out, B, T, H, ndir, workspace, workspace_bytes,
+    return bilstm_run(CELL_LSTM, false, gates, w_hh, cstate, out, B, T, H, ndir, workspace, workspace_bytes,
                       (cudaStream_t)stream);
 }
 
 extern "C" int b200asr_bilstm_bwd(float* gates, const float* w_hh, const float* cstate, const float* dout, int B,
                                   int T, int H, int ndir, void* workspace, size_t workspace_bytes,
                                   b200asr_stream stream) {
-    return bilstm_run(true, gates, w_hh, const_cast<float*>(cstate), const_cast<float*>(dout), B, T, H, ndir,
+    return bilstm_run(CELL_LSTM, true, gates, w_hh, const_cast<float*>(cstate), const_cast<float*>(dout), B, T, H, ndir,
+                      workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int b200asr_bigru_fwd(float* gates, const float* w_hh, float* hstate, float* out, int B, int T, int H,
+                                 int ndir, void* workspace, size_t workspace_bytes, b200asr_stream stream) {
+    return bilstm_run(CELL_GRU, false, gates, w_hh, hstate, out, B, T, H, ndir, workspace, workspace_bytes,
+                      (cudaStream_t)stream);
+}
+
+extern "C" int b200asr_bigru_bwd(float* gates, const float* w_hh, const float* hstate, const float* dout, int B,
+                                 int T, int H, int ndir, void* workspace, size_t workspace_bytes,
+                                 b200asr_stream stream) {
+    return bilstm_run(CELL_GRU, true, gates, w_hh, const_cast<float*>(hstate), const_cast<float*>(dout), B, T, H, ndir,
                       workspace, workspace_bytes, (cudaStream_t)stream);
 }
 

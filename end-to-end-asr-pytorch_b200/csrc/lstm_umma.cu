@@ -30,6 +30,7 @@
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "lstm_umma.h"
+#include "rnn_cell.cuh"
 
 namespace b200asr {
 namespace {
@@ -139,8 +140,8 @@ __global__ void ul_pack_fwd_kernel(const float* __restrict__ w, uint8_t* __restr
 // j = w / 4 (the unit quad), i.e. ONE cell (batch row 8q + lane/4, unit 4j + lane%4) per thread; warp UBP = publisher
 // (one lane: ONE gpu-scope fence + release per CTA and step, after the epilogue warps arrived on `pub`); warps
 // UBP+1 .. UBP+NC = control, one lane each, control warp c owns K atoms c, c+NC, ...
-template <int UBP>
-__global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_umma_kernel(UlParams p) {
+template <int CELL, int UBP>
+__device__ __forceinline__ void fwd_umma_body(const UlParams& p) {
     constexpr int N = 8 * UBP;            // B operand rows (gate columns, hi + lo copies)
     extern __shared__ __align__(1024) uint8_t smem[];
     const int H = p.H, T = p.T, NA = p.NA, UB = p.UB;
@@ -263,13 +264,11 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
                 pre.z += dgo[0] + (dgo[2] + ego[0]) * k;
                 pre.w += dgo[1] + (dgo[3] + ego[1]) * k;
             }
-            const float ig = sigmoidf_(pre.x);
-            const float fg = sigmoidf_(pre.y);
-            const float gg = tanhf(pre.z);
-            const float og = sigmoidf_(pre.w);
-            const float c = fmaf(fg, c_reg, ig * gg);
+            float c = c_reg;                              // c_t (LSTM) / h_t (GRU) after the cell
+            float4 gq;
+            cell_fwd<CELL>([&](int q) { return f4_at(pre, q); }, c, gq);
             c_reg = ok ? c : 0.f;
-            const float hq = ok ? og * tanhf(c) : 0.f;
+            const float hq = ok ? cell_h<CELL>(gq, c) : 0.f;
             if (step + 1 < T) {
                 // publish h_step as element (A row, k = ug) of the next A operand, fp16 hi / lo
                 uint8_t* dstimg = xb + (size_t)(step & 1) * img_bytes;
@@ -296,7 +295,7 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
             }
             // the stash / output stores of this step are issued during the NEXT step (after its MMAs): stores
             // in flight while the publisher runs its gpu-scope fence lengthen that fence by their L2 round trip
-            st_g = make_float4(ig, fg, gg, og);
+            st_g = gq;
             st_c = c;
             st_h = hq;
             st_row = rowbase;
@@ -309,6 +308,15 @@ __global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_um
             p.out[st_out] = st_h;
         }
     }
+}
+// the step kernels of the two cells (csrc/rnn_cell.cuh) on one body
+template <int UBP>
+__global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bilstm_fwd_umma_kernel(UlParams p) {
+    fwd_umma_body<CELL_LSTM, UBP>(p);
+}
+template <int UBP>
+__global__ void __launch_bounds__(32 * (UBP + 1 + UL_MAX_CTRL), 1) bigru_fwd_umma_kernel(UlParams p) {
+    fwd_umma_body<CELL_GRU, UBP>(p);
 }
 
 // =====================================================================================================================
@@ -392,8 +400,8 @@ __host__ __device__ inline size_t ulb_staging_bytes(int nub, int UB, int CS) {
 // A destination then polls nub / CS sources (one per cluster) instead of nub, and the L2 traffic per step drops CS x.
 // Warp roles: warps [0, 16) pointwise + MMA + drain; lane 0 of warp 17 loads W_hh.  Warps 16 and 18 .. 20 have no work
 // but stay in the block: __launch_bounds__ and ul_launch_bwd's occupancy check count them.
-template <int UB, int CS>
-__global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm_bwd_umma_kernel(UlParams p) {
+template <int CELL, int UB, int CS>
+__device__ __forceinline__ void bwd_umma_body(const UlParams& p) {
     constexpr int KS = (4 * UB) / 16;               // MMAs (k-steps of 16) per product and n-block
     // the 64 columns of a warpgroup's n-block start on a multiple of UB * CS units, so the aggregating rank of each
     // accumulator column group depends only on its offset inside the block
@@ -523,14 +531,7 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
             }
             float4 dg = make_float4(0.f, 0.f, 0.f, 0.f);
             if (ok) {
-                const float ig = gtv.x, fg = gtv.y, gg = gtv.z, og = gtv.w;
-                const float tc = tanhf(ct);
-                const float dc = dc_reg + dh * og * (1.f - tc * tc);
-                dg.x = dc * gg * ig * (1.f - ig);
-                dg.y = dc * cp * fg * (1.f - fg);
-                dg.z = dc * ig * (1.f - gg * gg);
-                dg.w = dh * tc * og * (1.f - og);
-                dc_reg = dc * fg;
+                cell_bwd<CELL>(gtv, ct, cp, dh, dc_reg, dg);
                 *reinterpret_cast<float4*>(p.gates + (row * H + ug) * 4) = dg;
             }
             if (step + 1 < T) {
@@ -658,6 +659,14 @@ __global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm
     }
     if (CS > 1) cluster_sync_all();                 // no peer accesses this block's shared memory after it exits
 }
+template <int UB, int CS>
+__global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bilstm_bwd_umma_kernel(UlParams p) {
+    bwd_umma_body<CELL_LSTM, UB, CS>(p);
+}
+template <int UB, int CS>
+__global__ void __launch_bounds__(32 * (ULB_EPI_WARPS + 1 + ULB_CTRL), 1) bigru_bwd_umma_kernel(UlParams p) {
+    bwd_umma_body<CELL_GRU, UB, CS>(p);
+}
 
 struct UlPlan {
     int UB, UBp, nub, nbg, ctas, NA, Bsub, nsplit;
@@ -695,7 +704,7 @@ int ul_plan(int B, int H, int ndir, UlPlan* out) {
 
 size_t ul_align(size_t x) { return (x + 255) / 256 * 256; }
 
-template <int UBP>
+template <int CELL, int UBP>
 int ul_launch_fwd(const UlPlan& pl, UlParams p, const float* w_hh, cudaStream_t stream) {
     {
         const long long n = (long long)p.ndir * pl.nub * 8 * UBP * p.H;
@@ -704,7 +713,7 @@ int ul_launch_fwd(const UlPlan& pl, UlParams p, const float* w_hh, cudaStream_t 
         ul_pack_fwd_kernel<UBP><<<blocks, 256, 0, stream>>>(w_hh, const_cast<uint8_t*>(p.wpack), p.H, pl.UB, p.ndir);
         B200_LAUNCH_CHECK("ul_pack_fwd_kernel");
     }
-    const void* fn = (const void*)bilstm_fwd_umma_kernel<UBP>;
+    const void* fn = CELL == CELL_GRU ? (const void*)bigru_fwd_umma_kernel<UBP> : (const void*)bilstm_fwd_umma_kernel<UBP>;
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
     int per_sm = 0;
     const int threads = 32 * (UBP + 1 + p.NC);
@@ -731,7 +740,14 @@ struct UlbPlan {
 int g_ulb_cs_cap = 0;              // test cap on CS (debug lstm mode bits 4..6; 0: none)
 bool g_ulb_coop_refused = false;   // the runtime refused a cooperative cluster launch: CS = 1 from then on
 
-const void* ulb_kernel(int UB, int CS) {
+const void* ulb_kernel(int cell, int UB, int CS) {
+    if (cell == CELL_GRU) {
+        if (UB == 16)
+            return CS == 4 ? (const void*)bigru_bwd_umma_kernel<16, 4>
+                           : CS == 2 ? (const void*)bigru_bwd_umma_kernel<16, 2> : (const void*)bigru_bwd_umma_kernel<16, 1>;
+        return CS == 4 ? (const void*)bigru_bwd_umma_kernel<8, 4>
+                       : CS == 2 ? (const void*)bigru_bwd_umma_kernel<8, 2> : (const void*)bigru_bwd_umma_kernel<8, 1>;
+    }
     if (UB == 16)
         return CS == 4 ? (const void*)bilstm_bwd_umma_kernel<16, 4>
                        : CS == 2 ? (const void*)bilstm_bwd_umma_kernel<16, 2> : (const void*)bilstm_bwd_umma_kernel<16, 1>;
@@ -757,9 +773,11 @@ void ulb_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, int c
 }
 
 // Clusters of CS blocks of this instance that the device holds at once (0 when it cannot be asked: no device, or a
-// runtime without the query).
+// runtime without the query).  The planner asks the LSTM instance for both cells: the GRU instances use no more
+// registers and the same shared memory (tests/test_host_gru_encoder.py checks it on the compiler's report), so the
+// plan and the variant queries are one for both cells.
 int ulb_max_clusters(int UB, int CS, int ctas, size_t smem) {
-    const void* fn = ulb_kernel(UB, CS);
+    const void* fn = ulb_kernel(CELL_LSTM, UB, CS);
     if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
         (void)cudaGetLastError();
         return 0;
@@ -823,7 +841,7 @@ int ulb_plan(int B, int H, int ndir, UlbPlan* out, bool cluster = true) {
 
 // One launch per row block.  A cooperative cluster launch that the runtime refuses runs nothing: the launches then
 // fall back to CS = 1 (and the planner never picks CS > 1 again in this process).
-template <int UB>
+template <int CELL, int UB>
 int ul_launch_bwd(UlbPlan pl, UlParams p, const float* w_hh, cudaStream_t stream) {
     {
         const long long n = (long long)p.ndir * pl.nub * 2 * p.H * 64;
@@ -833,7 +851,7 @@ int ul_launch_bwd(UlbPlan pl, UlParams p, const float* w_hh, cudaStream_t stream
         B200_LAUNCH_CHECK("ul_pack_bwd_kernel");
     }
     for (;;) {
-        const void* fn = ulb_kernel(UB, pl.CS);
+        const void* fn = ulb_kernel(CELL, UB, pl.CS);
         B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
         if (pl.CS == 1) {
             int per_sm = 0;
@@ -894,7 +912,7 @@ bool lstm_umma_fwd_variant(int B, int H, int ndir, int* ub, int* ubp, int* nspli
     return true;
 }
 
-int lstm_umma_bwd(float* gates, const float* w_hh, const float* cstate, const float* dout, int B, int T, int H, int ndir,
+int lstm_umma_bwd(int cell, float* gates, const float* w_hh, const float* cstate, const float* dout, int B, int T, int H, int ndir,
                   void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     UlbPlan pl;
     B200_REQUIRE(ulb_plan(B, H, ndir, &pl) == 0, "bilstm(umma bwd): unsupported shape B=%d H=%d ndir=%d", B, H, ndir);
@@ -909,8 +927,12 @@ int lstm_umma_bwd(float* gates, const float* w_hh, const float* cstate, const fl
     p.B = B; p.T = T; p.H = H; p.ndir = ndir; p.UB = pl.UB; p.nub = pl.nub; p.nbg = pl.nbg; p.NA = 0; p.NC = ULB_CTRL;
     p.strict = 0;
     p.b0 = 0; p.Bend = B;
-    if (pl.UB == 16) return ul_launch_bwd<16>(pl, p, w_hh, stream);
-    return ul_launch_bwd<8>(pl, p, w_hh, stream);
+    if (cell == CELL_GRU) {
+        if (pl.UB == 16) return ul_launch_bwd<CELL_GRU, 16>(pl, p, w_hh, stream);
+        return ul_launch_bwd<CELL_GRU, 8>(pl, p, w_hh, stream);
+    }
+    if (pl.UB == 16) return ul_launch_bwd<CELL_LSTM, 16>(pl, p, w_hh, stream);
+    return ul_launch_bwd<CELL_LSTM, 8>(pl, p, w_hh, stream);
 }
 
 size_t lstm_umma_workspace_bytes(int B, int H, int ndir) {
@@ -931,7 +953,7 @@ int lstm_umma_plan(int B, int H, int ndir, int* unit_block, int* batch_block, in
     return 0;
 }
 
-int lstm_umma_fwd(float* gates, const float* w_hh, float* cstate, float* out, int B, int T, int H, int ndir,
+int lstm_umma_fwd(int cell, float* gates, const float* w_hh, float* cstate, float* out, int B, int T, int H, int ndir,
                   void* workspace, size_t workspace_bytes, bool strict, cudaStream_t stream) {
     UlPlan pl;
     B200_REQUIRE(ul_plan(B, H, ndir, &pl) == 0, "bilstm(umma): unsupported shape B=%d H=%d ndir=%d", B, H, ndir);
@@ -947,10 +969,17 @@ int lstm_umma_fwd(float* gates, const float* w_hh, float* cstate, float* out, in
     p.NC = pl.NA < UL_MAX_CTRL ? pl.NA : UL_MAX_CTRL;
     p.strict = strict ? 1 : 0;
     p.b0 = 0; p.Bend = B;
+    if (cell == CELL_GRU) {
+        switch (pl.UBp) {
+            case 8: return ul_launch_fwd<CELL_GRU, 8>(pl, p, w_hh, stream);
+            case 12: return ul_launch_fwd<CELL_GRU, 12>(pl, p, w_hh, stream);
+            default: return ul_launch_fwd<CELL_GRU, 16>(pl, p, w_hh, stream);
+        }
+    }
     switch (pl.UBp) {
-        case 8: return ul_launch_fwd<8>(pl, p, w_hh, stream);
-        case 12: return ul_launch_fwd<12>(pl, p, w_hh, stream);
-        default: return ul_launch_fwd<16>(pl, p, w_hh, stream);
+        case 8: return ul_launch_fwd<CELL_LSTM, 8>(pl, p, w_hh, stream);
+        case 12: return ul_launch_fwd<CELL_LSTM, 12>(pl, p, w_hh, stream);
+        default: return ul_launch_fwd<CELL_LSTM, 16>(pl, p, w_hh, stream);
     }
 }
 

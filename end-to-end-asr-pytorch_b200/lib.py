@@ -47,6 +47,8 @@ SIGNATURES = {
     "b200asr_bilstm_uses_tcgen05": (c_int, [c_int, c_int, c_int]),
     "b200asr_bilstm_fwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_bilstm_bwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
+    "b200asr_bigru_fwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
+    "b200asr_bigru_bwd": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),
     "b200asr_debug_set_lstm_mode": (None, [c_int]),
     "b200asr_debug_lstm_variant": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_int)]),
     "b200asr_debug_lstm_cluster": (c_int, [c_int, c_int, c_int, c_int]),

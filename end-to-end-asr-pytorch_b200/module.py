@@ -1,8 +1,8 @@
 """Encoder / attention building blocks with the reference's constructor signatures and state_dict keys
 (/root/reference/src/module.py), computing through the b200asr kernels.
 
-  RNNLayer               -> persistent BiLSTM kernels (ops.bilstm) + f16x3 input/weight-grad GEMMs (csrc/gemm.cu;
-                            the cuBLAS 3xTF32 composition when the input width is not a multiple of 4)
+  RNNLayer               -> persistent BiLSTM / BiGRU kernels (ops.bilstm, ops.bigru) + f16x3 input/weight-grad GEMMs
+                            (csrc/gemm.cu; the cuBLAS 3xTF32 composition when the input width is not a multiple of 4)
   LocationAwareAttention -> fused single-launch attention step, one or more heads (ops.loc_attention_mem_step,
                             ops.loc_attention_heads_mem_step; the library ops for CPU tensors and unsupported shapes)
   CNNExtractor           -> its Conv1d(k 4, s 2) on the 3xTF32 GEMM kernel (ops.conv1d_k4s2p1)
@@ -80,10 +80,12 @@ class CNNExtractor(nn.Module):
 
 
 class RNNLayer(nn.Module):
-    """(Bi)LSTM + optional LayerNorm / dropout / time down-sampling / tanh projection (src/module.py:93-158).
+    """(Bi)LSTM or (Bi)GRU + optional LayerNorm / dropout / time down-sampling / tanh projection
+    (src/module.py:93-158).
 
-    `self.layer` is a torch.nn.LSTM used purely as the parameter container (identical state_dict keys); the
-    recurrence itself runs in the persistent sm_90a kernels."""
+    `self.layer` is a torch.nn.LSTM / torch.nn.GRU used as the parameter container (identical state_dict keys); the
+    recurrence itself runs in the persistent sm_90a kernels.  A GRU layer on CPU tensors, or with a width the kernels
+    have no plan for (H not a multiple of 16), runs through the nn.GRU module itself."""
 
     def __init__(self, input_dim, module, dim, bidirection, dropout, layer_norm, sample_rate, sample_style, proj):
         super().__init__()
@@ -100,8 +102,8 @@ class RNNLayer(nn.Module):
         self.module = module.upper()
         if self.module not in ("LSTM", "GRU"):
             raise NotImplementedError("RNN module %s (the reference accepts LSTM and GRU, src/module.py:112-113)" % module)
-        # LSTM: parameter container only, the recurrence runs in the persistent sm_90a kernels.  GRU (SURVEY.md 8(f)
-        # rank 4, no BASELINE config uses it): the library cuDNN layer, same state_dict keys as the reference.
+        # parameter container, same state_dict keys as the reference; the recurrence runs in the persistent sm_90a
+        # kernels (the GRU cell on the packed 4-slot layout, ops.BiGRUFn)
         self.layer = getattr(nn, self.module)(input_dim, dim, bidirectional=bidirection, num_layers=1, batch_first=True)
         if self.layer_norm:
             self.ln = nn.LayerNorm(rnn_out_dim)
@@ -119,6 +121,9 @@ class RNNLayer(nn.Module):
     def forward(self, input_x, x_len):
         if self.module == "LSTM":
             output = ops.bilstm(input_x, self.lstm_params(), self.ndir)
+        elif input_x.is_cuda and ops.rnn_layer_supported(input_x.shape[0], input_x.shape[1],
+                                                         self.layer.hidden_size, self.ndir):
+            output = ops.bigru(input_x, self.lstm_params(), self.ndir)
         else:
             output, _ = self.layer(input_x)
         if self.layer_norm:

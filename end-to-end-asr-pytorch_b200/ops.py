@@ -476,6 +476,120 @@ def mm3(a, b, out=None, bias=None, accumulate=False):
     return out
 
 
+def _rnn_layer_fwd(ctx, cell, x, ndir, w_ih, w_hh, bias):
+    """Forward of one (bi)directional LSTM or GRU layer on the 4-slot gate layout (BiLSTMFn, BiGRUFn): per direction
+    w_ih[d] [4H, I], w_hh[d] [4H, H] and bias[d] [4H], gate-major and detached -> (out [B, T, ndir*H], state stash
+    [ndir, B, T, H]: c (LSTM) / h (GRU) after every step).  Saves what _rnn_layer_bwd needs on ctx."""
+    lib = L.load()
+    x = _f32c(x)
+    B, T, I = x.shape
+    H = w_hh[0].shape[1]
+    dev = x.device
+    ws_bytes = lib.b200asr_bilstm_workspace_bytes(B, T, H, ndir)
+    if ws_bytes == 0:
+        raise L.B200AsrError("bi%s: no feasible decomposition for B=%d H=%d (H must be a multiple of 16)"
+                             % (cell.lower(), B, H))
+    perm = gate_perm(H, dev)
+    f16 = I % 4 == 0
+    # one operand of x serves both directions
+    xo = f16_split(x.view(B * T, I), B * T, I) if f16 else Split(x.view(B * T, I))
+    gates = torch.empty((ndir, B, T, H, 4), device=dev, dtype=torch.float32)
+    w_ih_p = []
+    for d in range(ndir):
+        wp = w_ih[d].index_select(0, perm)
+        bp = bias[d].index_select(0, perm)
+        if f16:
+            gemm_f16x3(xo, f16_split(wp, 4 * H, I), bias=bp, out=gates[d].view(B * T, 4 * H))
+        else:
+            mm3(xo, Split(wp).t(), out=gates[d].view(B * T, 4 * H), bias=bp)
+        w_ih_p.append(wp)
+    del xo
+    w_hh = torch.stack([_f32c(w) for w in w_hh]).contiguous()
+    cst = torch.empty((ndir, B, T, H), device=dev, dtype=torch.float32)
+    out = torch.empty((B, T, ndir * H), device=dev, dtype=torch.float32)
+    ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+    fn, name = (lib.b200asr_bilstm_fwd, "bilstm_fwd") if cell == "LSTM" else (lib.b200asr_bigru_fwd, "bigru_fwd")
+    # algorithmic bytes (SURVEY.md 8(d)): per step and direction read Gx[t] (16BH) + write h,c (8BH); W_hh once
+    with L.timed(name, ndir * (24 * B * H * T + 16 * H * H)):
+        L.check(fn(L.ptr(gates), L.ptr(w_hh), L.ptr(cst), L.ptr(out), B, T, H, ndir, L.ptr(ws), ws_bytes, L.stream()),
+                name)
+    ctx.cell = cell
+    ctx.ndir = ndir
+    ctx.dims = (B, T, I, H)
+    ctx.consumed = False
+    ctx.save_for_backward(x, gates, cst, out, w_hh, *w_ih_p)
+    return out, cst
+
+
+def _rnn_layer_bwd(ctx, dout):
+    """Backward of _rnn_layer_fwd -> (dx [B, T, I] or None, per direction (dw_ih [4H, I], dw_hh [4H, H], db [4H]) in
+    the gate-major 4-slot layout)."""
+    lib = L.load()
+    if ctx.consumed:
+        raise L.B200AsrError("%s.backward ran twice: the gate stash is overwritten in place"
+                             % ("BiLSTMFn" if ctx.cell == "LSTM" else "BiGRUFn"))
+    ctx.consumed = True
+    ndir = ctx.ndir
+    B, T, I, H = ctx.dims
+    x, gates, cst, out, w_hh = ctx.saved_tensors[:5]
+    w_ih_p = ctx.saved_tensors[5:5 + ndir]
+    dev = x.device
+    dout = _f32c(dout)
+    ws_bytes = lib.b200asr_bilstm_workspace_bytes(B, T, H, ndir)
+    ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+    fn, name = (lib.b200asr_bilstm_bwd, "bilstm_bwd") if ctx.cell == "LSTM" else (lib.b200asr_bigru_bwd, "bigru_bwd")
+    with L.timed(name, 2 * ndir * (24 * B * H * T + 16 * H * H)):
+        L.check(fn(L.ptr(gates), L.ptr(w_hh), L.ptr(cst), L.ptr(dout), B, T, H, ndir, L.ptr(ws), ws_bytes,
+                   L.stream()), name)
+    perm = gate_perm(H, dev)
+    need_dx = ctx.needs_input_grad[0]
+    dx2 = torch.empty((B * T, I), device=dev, dtype=torch.float32) if need_dx else None
+    f16 = I % 4 == 0
+    if f16:
+        xt = f16_split_t(x, I, B * T)
+        # dG (d(loss)/d(pre-activation), unit-major columns) of both directions read once: its transposed images,
+        # its row images and its column sums (the bias gradient)
+        gts, grow, gsum = f16_split_dg(gates.view(ndir, B * T, 4 * H), row_images=need_dx)
+        if need_dx:
+            # dX = sum_d dG_d . W_d as one contraction over both directions
+            gemm_f16x3(grow, f16_split_cat_t(w_ih_p, grow[0].shape[2] // ndir), out=dx2)
+            del grow
+    else:
+        xs = Split(x.view(B * T, I))
+    grads = []
+    for d in range(ndir):
+        g2 = gates[d].view(B * T, 4 * H)      # d(loss)/d(pre-activation), unit-major columns
+        hd = out[:, :, d * H:(d + 1) * H]
+        if f16:
+            # dW_ih = dG^T . X and dW_hh = dG^T . h_prev on transposed images (h_prev's written shifted by one step
+            # per utterance, zero at the sequence ends); rows written through the gate permutation by the epilogue.
+            gt = gts[d]
+            dw_ih = gemm_f16x3(gt, xt, permute_rows=True, name="gemm_f16_nt")
+            ht = f16_split_t(hd, H, T, batches=B, ld=ndir * H, bstride=T * ndir * H, shift=(-1 if d == 0 else 1))
+            dw_hh = gemm_f16x3(gt, ht, permute_rows=True, name="gemm_f16_nt")
+            del gt, ht
+        else:
+            dG = Split(g2)
+            if need_dx:
+                mm3(dG, Split(w_ih_p[d]), out=dx2, accumulate=(d > 0))
+            dw_ih = torch.empty((4 * H, I), device=dev, dtype=torch.float32)
+            dw_ih.index_copy_(0, perm, mm3(dG.t(), xs))
+            # h_{prev}: the hidden state of the previous step of this direction (zero at its first step)
+            hprev = torch.zeros((B, T, H), device=dev, dtype=torch.float32)
+            if T > 1:
+                if d == 0:
+                    hprev[:, 1:] = hd[:, :-1]
+                else:
+                    hprev[:, :-1] = hd[:, 1:]
+            dw_hh = torch.empty((4 * H, H), device=dev, dtype=torch.float32)
+            dw_hh.index_copy_(0, perm, mm3(dG.t(), Split(hprev.view(B * T, H))))
+            del dG, hprev
+        db = torch.empty((4 * H,), device=dev, dtype=torch.float32)
+        db.index_copy_(0, perm, gsum[d] if f16 else g2.sum(0))
+        grads.append((dw_ih, dw_hh, db))
+    return (dx2.view(B, T, I) if need_dx else None), grads
+
+
 class BiLSTMFn(Function):
     """One (bi)directional LSTM layer over zero-padded frames, zero initial state (src/module.py:129-132).
 
@@ -487,115 +601,60 @@ class BiLSTMFn(Function):
 
     @staticmethod
     def forward(ctx, x, ndir, *params):
-        lib = L.load()
         sink = None
         if params and isinstance(params[-1], CStateSink):
             sink, params = params[-1], params[:-1]
         assert len(params) == 4 * ndir
-        x = _f32c(x)
-        B, T, I = x.shape
-        H = params[1].shape[1]
-        dev = x.device
-        ws_bytes = lib.b200asr_bilstm_workspace_bytes(B, T, H, ndir)
-        if ws_bytes == 0:
-            raise L.B200AsrError("bilstm: no feasible decomposition for B=%d H=%d (H must be a multiple of 16)" % (B, H))
-        perm = gate_perm(H, dev)
-        f16 = I % 4 == 0
-        # one operand of x serves both directions
-        xo = f16_split(x.view(B * T, I), B * T, I) if f16 else Split(x.view(B * T, I))
-        gates = torch.empty((ndir, B, T, H, 4), device=dev, dtype=torch.float32)
-        w_ih_p = []
-        for d in range(ndir):
-            w_ih, w_hh, b_ih, b_hh = params[4 * d:4 * d + 4]
-            wp = w_ih.detach().index_select(0, perm)
-            bp = (b_ih.detach() + b_hh.detach()).index_select(0, perm)
-            if f16:
-                gemm_f16x3(xo, f16_split(wp, 4 * H, I), bias=bp, out=gates[d].view(B * T, 4 * H))
-            else:
-                mm3(xo, Split(wp).t(), out=gates[d].view(B * T, 4 * H), bias=bp)
-            w_ih_p.append(wp)
-        del xo
-        w_hh = torch.stack([_f32c(params[4 * d + 1].detach()) for d in range(ndir)]).contiguous()
-        cst = torch.empty((ndir, B, T, H), device=dev, dtype=torch.float32)
-        out = torch.empty((B, T, ndir * H), device=dev, dtype=torch.float32)
-        ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
-        # algorithmic bytes (SURVEY.md 8(d)): per step and direction read Gx[t] (16BH) + write h,c (8BH); W_hh once
-        with L.timed("bilstm_fwd", ndir * (24 * B * H * T + 16 * H * H)):
-            L.check(lib.b200asr_bilstm_fwd(L.ptr(gates), L.ptr(w_hh), L.ptr(cst), L.ptr(out), B, T, H, ndir,
-                                           L.ptr(ws), ws_bytes, L.stream()), "bilstm_fwd")
+        out, cst = _rnn_layer_fwd(ctx, "LSTM", x, ndir, [params[4 * d].detach() for d in range(ndir)],
+                                  [params[4 * d + 1].detach() for d in range(ndir)],
+                                  [params[4 * d + 2].detach() + params[4 * d + 3].detach() for d in range(ndir)])
         if sink is not None:
             sink.cstate = cst
-        ctx.ndir = ndir
-        ctx.dims = (B, T, I, H)
         ctx.tail = (None,) if sink is not None else ()
-        ctx.consumed = False
-        ctx.save_for_backward(x, gates, cst, out, w_hh, *w_ih_p)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        lib = L.load()
-        if ctx.consumed:
-            raise L.B200AsrError("BiLSTMFn.backward ran twice: the gate stash is overwritten in place")
-        ctx.consumed = True
-        ndir = ctx.ndir
-        B, T, I, H = ctx.dims
-        x, gates, cst, out, w_hh = ctx.saved_tensors[:5]
-        w_ih_p = ctx.saved_tensors[5:5 + ndir]
-        dev = x.device
-        dout = _f32c(dout)
-        ws_bytes = lib.b200asr_bilstm_workspace_bytes(B, T, H, ndir)
-        ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
-        with L.timed("bilstm_bwd", 2 * ndir * (24 * B * H * T + 16 * H * H)):
-            L.check(lib.b200asr_bilstm_bwd(L.ptr(gates), L.ptr(w_hh), L.ptr(cst), L.ptr(dout), B, T, H, ndir,
-                                           L.ptr(ws), ws_bytes, L.stream()), "bilstm_bwd")
-        perm = gate_perm(H, dev)
-        need_dx = ctx.needs_input_grad[0]
-        dx2 = torch.empty((B * T, I), device=dev, dtype=torch.float32) if need_dx else None
-        f16 = I % 4 == 0
-        if f16:
-            xt = f16_split_t(x, I, B * T)
-            # dG (d(loss)/d(pre-activation), unit-major columns) of both directions read once: its transposed images,
-            # its row images and its column sums (the bias gradient)
-            gts, grow, gsum = f16_split_dg(gates.view(ndir, B * T, 4 * H), row_images=need_dx)
-            if need_dx:
-                # dX = sum_d dG_d . W_d as one contraction over both directions
-                gemm_f16x3(grow, f16_split_cat_t(w_ih_p, grow[0].shape[2] // ndir), out=dx2)
-                del grow
-        else:
-            xs = Split(x.view(B * T, I))
+        dx, per_dir = _rnn_layer_bwd(ctx, dout)
         grads = []
-        for d in range(ndir):
-            g2 = gates[d].view(B * T, 4 * H)      # d(loss)/d(pre-activation), unit-major columns
-            hd = out[:, :, d * H:(d + 1) * H]
-            if f16:
-                # dW_ih = dG^T . X and dW_hh = dG^T . h_prev on transposed images (h_prev's written shifted by one step
-                # per utterance, zero at the sequence ends); rows written through the gate permutation by the epilogue.
-                gt = gts[d]
-                dw_ih = gemm_f16x3(gt, xt, permute_rows=True, name="gemm_f16_nt")
-                ht = f16_split_t(hd, H, T, batches=B, ld=ndir * H, bstride=T * ndir * H, shift=(-1 if d == 0 else 1))
-                dw_hh = gemm_f16x3(gt, ht, permute_rows=True, name="gemm_f16_nt")
-                del gt, ht
-            else:
-                dG = Split(g2)
-                if need_dx:
-                    mm3(dG, Split(w_ih_p[d]), out=dx2, accumulate=(d > 0))
-                dw_ih = torch.empty((4 * H, I), device=dev, dtype=torch.float32)
-                dw_ih.index_copy_(0, perm, mm3(dG.t(), xs))
-                # h_{prev}: the hidden state of the previous step of this direction (zero at its first step)
-                hprev = torch.zeros((B, T, H), device=dev, dtype=torch.float32)
-                if T > 1:
-                    if d == 0:
-                        hprev[:, 1:] = hd[:, :-1]
-                    else:
-                        hprev[:, :-1] = hd[:, 1:]
-                dw_hh = torch.empty((4 * H, H), device=dev, dtype=torch.float32)
-                dw_hh.index_copy_(0, perm, mm3(dG.t(), Split(hprev.view(B * T, H))))
-                del dG, hprev
-            db = torch.empty((4 * H,), device=dev, dtype=torch.float32)
-            db.index_copy_(0, perm, gsum[d] if f16 else g2.sum(0))
+        for dw_ih, dw_hh, db in per_dir:
             grads += [dw_ih, dw_hh, db, db.clone()]
-        return (dx2.view(B, T, I) if need_dx else None, None, *grads, *ctx.tail)
+        return (dx, None, *grads, *ctx.tail)
+
+
+class BiGRUFn(Function):
+    """One (bi)directional GRU layer over zero-padded frames, zero initial state (src/module.py:129-132, the nn.GRU
+    branch): the BiLSTM layer with the GRU cell.
+
+    forward(x[B,T,I], ndir, w_ih_0, w_hh_0, b_ih_0, b_hh_0 [, ..._1]) -> out[B,T,ndir*H], parameters in nn.GRU's
+    layout (gates r, z, n).  Each direction is packed into the 4-slot layout of pack_decoder_weights("GRU"), the one
+    packing rule of the GRU speller and encoder: W_ih4 = [W_ir; W_iz; W_in; 0], W_hh4 = [W_hr; W_hz; 0; W_hn], bias
+    (b_ir + b_hr, b_iz + b_hz, b_in, b_hn), so that the input projection and h . W_hh4^T yield (r, z, gi_n, gh_n).  The
+    recurrence is b200asr_bigru_fwd / _bwd; the layer GEMMs, dX and the weight gradients are BiLSTMFn's on the 4H rows
+    (the zero slots cost 4/3 of a GRU layer's contraction FLOPs), mapped back by unpack_decoder_grads("GRU").
+    """
+
+    @staticmethod
+    def forward(ctx, x, ndir, *params):
+        assert len(params) == 4 * ndir
+        I = params[0].shape[1]
+        w_ih, w_hh, bias = [], [], []
+        for d in range(ndir):
+            wcat, b = pack_decoder_weights("GRU", *(p.detach() for p in params[4 * d:4 * d + 4]))
+            w_ih.append(wcat[:, :I])
+            w_hh.append(wcat[:, I:])
+            bias.append(b)
+        out, _ = _rnn_layer_fwd(ctx, "GRU", x, ndir, w_ih, w_hh, bias)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        dx, per_dir = _rnn_layer_bwd(ctx, dout)
+        I = ctx.dims[2]
+        grads = []
+        for dw_ih, dw_hh, db in per_dir:
+            grads += unpack_decoder_grads("GRU", torch.cat([dw_ih, dw_hh], 1), db, I)
+        return (dx, None, *grads)
 
 
 class CStateSink:
@@ -606,6 +665,16 @@ class CStateSink:
 
 def bilstm(x, lstm_params, ndir, sink=None):
     return BiLSTMFn.apply(x, ndir, *lstm_params, *((sink,) if sink is not None else ()))
+
+
+def bigru(x, gru_params, ndir):
+    """One (bi)directional GRU layer; gru_params = nn.GRU's (weight_ih, weight_hh, bias_ih, bias_hh) per direction."""
+    return BiGRUFn.apply(x, ndir, *gru_params)
+
+
+def rnn_layer_supported(B, T, H, ndir):
+    """True when the persistent recurrence kernels have a plan for this layer (H a multiple of 16)."""
+    return L.load().b200asr_bilstm_workspace_bytes(B, T, H, ndir) != 0
 
 
 # ----------------------------------------------------------------------------------------------------------

@@ -152,6 +152,26 @@ B200ASR_API int b200asr_bilstm_fwd(float* gates, const float* w_hh, float* cstat
 B200ASR_API int b200asr_bilstm_bwd(float* gates, const float* w_hh, const float* cstate, const float* dout, int B, int T,
                        int H, int ndir, void* workspace, size_t workspace_bytes, b200asr_stream stream);
 
+/* ---- K7/K8 with a GRU cell: persistent (Bi)GRU recurrence -----------------------------------------------------
+ * replaces the time loop inside torch.nn.GRU as used by src/module.py:112-113,129-132 (the nn.GRU branch: one layer,
+ * batch_first, zero initial state, run over the padded frames).  Same kernels, plan, variants and workspace as the
+ * BiLSTM above (b200asr_bilstm_workspace_bytes / _plan / b200asr_debug_lstm_variant answer for both cells); only the
+ * pointwise cell differs.  The layer's weights are packed into four gate slots per unit, as ops.pack_decoder_weights
+ * ("GRU") packs them:
+ *   gates  [ndir, B, T, H, 4]  in : (gi_r + gh_r, gi_z + gh_z, gi_n, gh_n) of the input projection, i.e. x.W_ih4^T + b4
+ *                                   with W_ih4 = [W_ir; W_iz; W_in; 0] and b4 = (b_ir + b_hr, b_iz + b_hz, b_in, b_hn)
+ *                              out: (r, z, n, gh_n) with gh_n = h_{t-1}.W_hn^T + b_hn (stash for the backward pass)
+ *   w_hh   [ndir, 4H, H]       packed [W_hr; W_hz; 0; W_hn] (gate-major rows g*H + j, slot 2 zero)
+ *   hstate [ndir, B, T, H]     out: h after every step (stash; the backward reads h_{t-1} from it)
+ *   out    [B, T, ndir*H]      out: hidden states (the layer output)
+ * r = sigmoid, z = sigmoid, n = tanh(gi_n + r.gh_n), h = (h_prev - n).z + n in ATen's expression order.
+ * backward: gates in = stash, out = dG = (d pre_r, d pre_z, d gi_n, d gh_n) in the same layout; dout [B, T, ndir*H].
+ * Limits as for the BiLSTM (H a multiple of 16).                                                                  */
+B200ASR_API int b200asr_bigru_fwd(float* gates, const float* w_hh, float* hstate, float* out, int B, int T, int H, int ndir,
+                      void* workspace, size_t workspace_bytes, b200asr_stream stream);
+B200ASR_API int b200asr_bigru_bwd(float* gates, const float* w_hh, const float* hstate, const float* dout, int B, int T,
+                      int H, int ndir, void* workspace, size_t workspace_bytes, b200asr_stream stream);
+
 
 /* ---- K13: one LSTM cell step (decoder, src/asr.py:214-221) -------------------------------------------------
  * preact [B, 4H] gate-major (i,f,g,o) = x.W_ih^T + h.W_hh^T + biases; gates [B,4H] activated (stash).        */
